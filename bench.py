@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """bench.py -- EI candidates/sec of the GP-EI chooser hot path, and chooser.next() wall-ms (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload NAME] [--dump-outputs DIR]
 
 A "step" is one pass of ``ei_over_hypers`` (chooser/GPEIOptChooser.py:331-341 of the reference) over the
 whole candidate grid for all S hyper-samples: K build -> Cholesky -> explicit inverse + alpha -> cross-covariance
-generator -> tcgen05 predict GEMM (3xFP16 scaled split) -> EI sweep (-> all-reduce of the per-candidate EI sum when
+generator -> wgmma predict GEMM (3xFP16 scaled split) -> EI sweep (-> all-reduce of the per-candidate EI sum when
 N > 1) -> argmax.
 
   value : M / step-time with X, candidates, values and hyper-samples already resident in HBM.
@@ -13,9 +13,8 @@ N > 1) -> argmax.
           host numpy in, (M, S) float64 EI matrix out, then the host argmax of the mean), host<->device copies inside
           the timed region, --steps iterations.
   roofline     : the dominant kernel (tc::predict_tc_kernel, the N^2*M triangular-solve term as a GEMM against the
-                 explicit inverse): algorithmic flops / its CUDA-event time vs the measured dense bf16 tensor peak
-                 (MEASURED_PEAKS.json); traffic = DRAM bytes per launch read from the committed ncu summary
-                 profiles/r02_predict_tc_traffic.json (bench.py never runs under a profiler).
+                 explicit inverse): algorithmic flops / its CUDA-event time vs the dense bf16 tensor peak
+                 (MEASURED_PEAKS.json when present, else the H100 SXM data-sheet figure).
   cpu_baseline : the oracle port (oracle.gp_oracle.compute_ei: the reference's own numpy/scipy operation sequence,
                  GPEIOptChooser.py:527-556) timed on this box's host cores -- BLAS threads pinned to all of them, the same
                  at every --gpus N -- on a bounded sample and extrapolated linearly (the reference loop is exactly
@@ -24,6 +23,9 @@ N > 1) -> argmax.
   next  : chooser.next() wall-ms through the plugin API at the SAME workload, steady state (no burn-in), with the phase
           split (MCMC / grid pass 1 / L-BFGS refinement / grid pass 2) and the CPU port's time as counts x unit times.
   --impl reference : the CPU implementation as its own arm (rank 0 only).
+  --dump-outputs DIR : after the timed steps, what the last timed step returned -- the per-candidate EI sum over all
+          hyper-samples (ei_sum.npy, float64, M values) and the proposed candidate (argmax.npy) -- so that two builds can be
+          compared output for output (the inputs are seeded: identical from run to run for the same arguments).
 
 Multi-GPU: hyper-samples are sharded round-robin over ranks (total work fixed -> "scaling": "strong"); the
 only exchange is one NCCL all-reduce of M floats.
@@ -90,29 +92,18 @@ def flops_per_pair(N, D):
     return float(N) * N + 2.0 * N * D + 4.0 * N + 25.0 * N + 40.0
 
 
-def ncu_traffic(workload, impl, world, launches_per_step):
-    """DRAM bytes per launch of the dominant kernel from the committed ncu summary (which names its capture commit)."""
-    p = os.path.join(ROOT, "profiles", "r02_predict_tc_traffic.json")
-    if impl != "tc" or world != 1 or not os.path.exists(p):
-        return None, None
-    d = json.load(open(p))
-    w = d.get("workloads", {}).get(workload)
-    if not w:
-        return None, None
-    return float(w["dram_bytes_per_step"]) / max(1, launches_per_step), "profiles/r02_predict_tc_traffic.json @ %s" % d.get("commit")
-
-
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tensor_burst=d["bf16_tflops"], tensor_sustained=d["bf16_tflops_sustained"],
                     src="MEASURED_PEAKS.json")
-    return dict(hbm=6650.0, tensor_burst=1590.0, tensor_sustained=1400.0, src="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- a ceiling, not a measured rate
+    return dict(hbm=3350.0, tensor_burst=989.0, tensor_sustained=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler(object):
-    """nvidia-smi clock / throttle-reason samples during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clock / throttle-reason samples during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -258,16 +249,15 @@ def run_b200_arm(args, D, N, M, S):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: the product arm needs a CUDA device (B200, sm_100a) -- there is no CPU fallback; "
+        raise SystemExit("bench.py: the product arm needs a CUDA device (H100, sm_90a) -- there is no CPU fallback; "
                          "the CPU arm is `--impl reference`")
     torch.cuda.set_device(local)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda:%d" % local))
         # The all-cores thread setting at the top of this file is for the CPU arm (rank 0 alone).  Here every rank runs host
         # code of its own (dtype conversions of the uploads are OpenMP loops in torch): N ranks x all cores oversubscribes the
-        # host N times.  The plugin call measured 148 ms at 2 GPUs and 139 ms at 8 against 128 / 34 ms of device time -- growing
-        # with the rank count, which is what spinning OpenMP teams on an oversubscribed host look like (not re-measured at 8
-        # GPUs after this change: the round's GPU budget was spent).  Each rank gets its share of the cores.
+        # host N times, and spinning OpenMP teams then slow the plugin call down as the rank count grows.  Each rank gets
+        # its share of the cores.
         share = max(1, _CORES // world)
         torch.set_num_threads(share)
         try:
@@ -304,7 +294,7 @@ def run_b200_arm(args, D, N, M, S):
             ei_sum = torch.zeros((ldm,), dtype=torch.float64, device=eng.device)
         parallel.allreduce_sum_(ei_sum)
         idx, _ = eng.topk(ei_sum, M, 1)
-        return idx
+        return idx, ei_sum
 
     # ---- e2e leg: the plugin call.  GPEIOptChooserB200.ei_over_hypers is the drop-in for OPT:331-341; the per-second
     # plugin's method reproduces the reference's column-0-only early return (PSEC:302), so that workload goes through the
@@ -364,8 +354,12 @@ def run_b200_arm(args, D, N, M, S):
         step_resident()
     eng.check_deferred()
     sampler.mark_begin()
-    ms, _, launches, stages, idx = timed(step_resident, args.steps, with_timers=True)
+    ms, _, launches, stages, (idx, ei_sum) = timed(step_resident, args.steps, with_timers=True)
     eng.check_deferred()
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "ei_sum.npy"), ei_sum[:M].double().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "argmax.npy"), idx[:1].double().cpu().numpy())
     clocks = sampler.stop() if rank == 0 else None
     ms_per_step = ms / args.steps
     value = M / (ms_per_step * 1e-3)
@@ -393,7 +387,7 @@ def run_b200_arm(args, D, N, M, S):
         kms_total, cnt_v = span[kname]
         kms_step = kms_total / args.steps                       # all launches of the dominant kernel in one step
         n_launch_step = max(1, cnt_v // args.steps)
-        # algorithmic flops handled by that kernel per step (SURVEY 8d): the N^2 triangular-solve term for the tcgen05
+        # algorithmic flops handled by that kernel per step (SURVEY 8d): the N^2 triangular-solve term for the wgmma
         # kernel (the cross-covariance is a separate kernel there), the whole per-pair count for the fused SIMT kernel
         alg = (float(N) * N if impl == "tc" else flops_per_pair(N, D)) * pairs_local
         achieved = alg / (kms_step * 1e-3) / 1e12 if kms_step > 0 else None
@@ -401,19 +395,17 @@ def run_b200_arm(args, D, N, M, S):
         for nm in ("kxt_kernel", "trtri_kernel", "linv_pack_f16"):
             if span[nm][1]:
                 other[nm + "_ms_per_step"] = span[nm][0] / args.steps
-        traffic, traffic_src = ncu_traffic(args.workload, impl, world, n_launch_step)
-        roof = {"kernel": "smk::tc::predict_tc_kernel (tcgen05.mma kind::f16, 3xFP16 scaled split, fp32 accumulate)" if impl == "tc"
+        roof = {"kernel": "smk::tc::predict_tc_kernel (wgmma f16, 3xFP16 scaled split, fp32 accumulate)" if impl == "tc"
                 else "smk::predict_kernel<float> (SIMT FMA)",
                 "bound": "tensor", "achieved": achieved, "peak": pk["tensor_sustained"], "unit": "TFLOP/s",
                 "frac": (achieved / pk["tensor_sustained"]) if achieved else None,
-                "traffic": traffic, "traffic_source": traffic_src,
                 "peak_source": pk["src"] + " bf16 dense, sustained (kernel timed inside a long step)",
                 "algorithmic_flops_per_launch": alg / n_launch_step, "launches_per_step": n_launch_step,
                 "kernel_ms_per_launch": kms_step / n_launch_step, "kernel_ms_per_step": kms_step,
                 "note": "fp32-accurate results need 3 fp16 MMAs per product (hi*hi + hi*lo + lo*hi, operands scaled by exact "
                         "powers of two): 3 bf16-equivalent tensor flops per algorithmic flop, so 1/3 = 0.333 of the "
                         "bf16 peak is this formulation's ceiling"
-                        if impl == "tc" else "float32 SIMT FMA path (B200 fp32 vector peak ~74 TFLOP/s)",
+                        if impl == "tc" else "float32 SIMT FMA path (H100 SXM data sheet: 67 TFLOP/s FP32)",
                 "stage_ms_per_step": dict({k: v / args.steps for k, v in stages.items()}, **other)}
         out = {"metric": "EI candidates/sec", "value": value, "unit": "candidates/s", "n_gpus": world,
                "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": ms_per_step,
@@ -421,7 +413,7 @@ def run_b200_arm(args, D, N, M, S):
                "data": "synthetic",
                "config": {"workload": "%s D=%d N=%d M=%d S=%d %s" % (args.workload, D, N, M, S, KIND),
                           "parallelism": "hyper-samples round-robin over %d GPU(s), one all-reduce of M floats" % world,
-                          "l2": "working set (factors %.1f GB per rank) >> 126 MB L2, no flush needed"
+                          "l2": "working set (factors %.1f GB per rank) >> 50 MB L2, no flush needed"
                                 % (Sl * (((N + 127) // 128) * 128) ** 2 * 4 / 1e9),
                           "pairs_per_sec": value * S, "argmax": int(idx.cpu()[0]), "argmax_e2e": best_idx},
                "e2e": {"value": M / (e2e_ms * 1e-3), "unit": "candidates/s", "ms_per_step": e2e_ms, "steps": args.steps,
@@ -506,6 +498,8 @@ def main():
     ap.add_argument("--no-next", action="store_true", help="skip the chooser.next() wall-ms leg")
     ap.add_argument("--next-calls", type=int, default=1, help="timed next() calls")
     ap.add_argument("--next-cpu", action="store_true", help="also run the CPU port of next() for real (slow)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs (ei_sum.npy, argmax.npy) to DIR")
     args = ap.parse_args()
     D, N, M, S = WORKLOADS[args.workload]
     if args.samples:

@@ -1,5 +1,5 @@
 /*
- * spearmint_b200.h -- C ABI of the B200-native GP-EI hot path (libspearmint_b200.so).
+ * spearmint_b200.h -- C ABI of the H100-native (sm_90a) GP-EI hot path (libspearmint_b200.so).
  *
  * Drop-in boundary: the reference (JasperSnoek/spearmint) is pure Python and binds nothing
  * native on this path, so the "FFI" a maintainer would add is a ctypes binding inside a
@@ -124,7 +124,7 @@ int smk_predict_f64(int kind, int N, int Npad, int M, int D, int S, const double
                     const double* winv, const double* alpha, double* mu, double* var, int ldm,
                     void* workspace, size_t workspace_bytes, void* stream);
 
-/* ---- (4-tc) fused predict on the tensor cores (tcgen05 + TMEM + TMA; float32 in/out, 3 x FP16 split products
+/* ---- (4-tc) fused predict on the tensor cores (wgmma + TMA, register accumulators; float32 in/out, 3 x FP16 split products
  *      with exact power-of-two operand scaling, fp32 accumulation)
  * Same outputs as smk_predict_f32 (OPT:536, 544, 547-548).  Steps, so that the factor-only part is done once:
  *   smk_trtri_split_f32 : Linv = L^-1 (explicit inverse of the blocked factor) as a tf32 hi / lo pair of float arrays,
@@ -132,7 +132,7 @@ int smk_predict_f64(int kind, int N, int Npad, int M, int D, int S, const double
  *   smk_linv_pack_f16   : the GEMM operand copy of Linv: per-sample scale 2^linv_exp[s] (largest |entry| -> [2^14, 2^15))
  *                         and the round-to-nearest fp16 (hi, lo) pair, each [S][Np][Np] halves.
  *                         linv_exp: [2*S] ints (first S: exponents, rest scratch).
- *   smk_predict_tc_f32  : cross-covariance (candidate-major, fp16 hi/lo) -> D = Kxt * Linv^T on tcgen05 -> var, mu.
+ *   smk_predict_tc_f32  : cross-covariance (candidate-major, fp16 hi/lo) -> D = Kxt * Linv^T on wgmma -> var, mu.
  * alpha: [S][Npad_alpha] (first right-hand side).  dbg_beta (tests only, may be NULL): [S][Mc][Np] dump of
  * beta^T for a single-chunk call.
  * z (may be NULL): [S][Np], z = Linv (y - mean) -- the `tmp` output of smk_linv_alpha_f32.  With z the predictive mean is
@@ -146,8 +146,8 @@ int smk_trtri_split_f32(int Npad, int Np, int S, const float* L, const float* wi
                         float* linv_lo, void* workspace, size_t workspace_bytes, void* stream);
 /* Tensor-core variants of the N^3 steps (float32, 3xTF32, same outputs):
  *   smk_potrf_lower_batched_tc_f32 : left-looking blocked Cholesky, the rank-(jb*128) update of every block-column pair
- *       runs on tcgen05 (workspace: 2*S*Npad*Npad floats for the tf32 hi/lo copies of the finished panels).
- *   smk_trtri_split_tc_f32 : L^-1 by row blocks, X[K,:] = -(W_KK L[K,:]) X on tcgen05; writes linv_hi/linv_lo like
+ *       runs on wgmma (workspace: 2*S*Npad*Npad floats for the tf32 hi/lo copies of the finished panels).
+ *   smk_trtri_split_tc_f32 : L^-1 by row blocks, X[K,:] = -(W_KK L[K,:]) X on wgmma; writes linv_hi/linv_lo like
  *       smk_trtri_split_f32 (workspace: smk_trtri_tc_workspace_bytes).                                          */
 int smk_potrf_lower_batched_tc_f32(int Npad, int S, float* A, float* winv, int* info, void* workspace,
                                    size_t workspace_bytes, void* stream);
@@ -174,11 +174,11 @@ int smk_tc_guard_f32(int N, int Npad, int Np, int S, const float* L, const float
                      void* workspace, size_t workspace_bytes, void* stream);
 size_t smk_predict_tc_workspace_bytes(int Np, int M, int S, int F);
 /* F > 1 with alpha_f [S][F][Npad_alpha] and mu_f [S][F][ldm] non-NULL: additionally the fantasy means
- * mu_f[s][f][j] = cov(X, C_j)' alpha_f[s][f] + mean[s]  (OPT:609) as a second tcgen05 GEMM on the same Kxt chunk. */
+ * mu_f[s][f][j] = cov(X, C_j)' alpha_f[s][f] + mean[s]  (OPT:609) as a second wgmma GEMM on the same Kxt chunk. */
 /* The cross-covariance operand generator on its own (cov(comp, cand), OPT:536, and the mean OPT:544), one chunk:
  * k_h16 / k_l16: [S][ceil128(M)][Np] halves = amp2 k(X_n, C_c) * 2^ea as an fp16 (hi, lo) pair, ea = 15 - ceil(log2(
- * amp2 (1 + 1e-6) 1.00001));  mu: [S][ldm].  impl 0: packed-float32 SIMT kernel (any D, S); impl 1: tensor-core kernel
- * (q = (x - c)^2 once per pair, contraction over dimensions for all samples on tcgen05; D <= 32, S <= 64, else -1).  */
+ * amp2 (1 + 1e-6) 1.00001));  mu: [S][ldm].  impl 0: SIMT kernel (any D, S); impl 1: tensor-core kernel
+ * (q = (x - c)^2 once per pair, contraction over dimensions for all samples on wgmma; D <= 32, S <= 64, else -1).  */
 size_t smk_kxt_pack_workspace_bytes(int Np, int M, int S);
 /* debug only: clock64() stamps of the first 64 tiles of CTA 0 of the last impl-1 launch made with SMK_KXT_TIMELINE=1
  * ([tile][8]: production start / end, issuer arrives / operands+accumulator ready / committed, epilogue waits / accumulator

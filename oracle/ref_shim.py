@@ -4,10 +4,9 @@ Nothing is copied: the Python-2 files under ``/root/reference`` are read at run 
 passed through a handful of mechanical py2->py3 regex rewrites (SURVEY.md section 8(c)) and
 ``exec``-ed into fresh module objects.  It exists so that
 
-  * ``tests/golden/make_golden.py`` can freeze golden input/output vectors of the real
-    reference (``gp.py``, ``GPEIOptChooser.py``, ``GPEIperSecChooser.py``, ``GPEIChooser.py``),
-  * ``tests/test_oracle_vs_reference.py`` can pin ``oracle/gp_oracle.py`` (the numpy
-    restatement) directly against the reference whenever ``/root/reference`` is present.
+  * ``tests/golden/make_golden*.py`` can freeze golden input/output vectors of the real
+    reference (``gp.py``, ``GPEIOptChooser.py``, ``GPEIperSecChooser.py``, ``GPEIChooser.py``,
+    ``sobol_lib.py``) that the tests compare against.
 
 ``/root/reference`` does not exist on the GPU box, so nothing imported by ``-m gpu`` tests,
 ``__graft_entry__.smoke()`` or ``bench.py`` may depend on this file at run time.
@@ -98,14 +97,3 @@ def load():
                    OPT=opt, PSEC=psec, GPEI=gpei)
     return _loaded
 
-
-def load_lite():
-    """The reference's spearmint-lite controller (spearmint-lite/spearmint-lite.py) with its own ExperimentGrid,
-    executed under the same py3 rewrites.  Returns the module (main_controller, GridMap...)."""
-    load()
-    lite_dir = os.path.join(REF_ROOT, "spearmint-lite")
-    if "ExperimentGrid" not in sys.modules or not getattr(sys.modules["ExperimentGrid"], "_lite", False):
-        sys.modules["sobol_lib"] = _exec_module("sobol_lib", os.path.join(lite_dir, "sobol_lib.py"))
-        eg = _exec_module("ExperimentGrid", os.path.join(lite_dir, "ExperimentGrid.py"))
-        eg._lite = True
-    return _exec_module("spearmint_lite", os.path.join(lite_dir, "spearmint-lite.py"))

@@ -1,9 +1,9 @@
-"""In-tree build of libspearmint_b200.so with nvcc for sm_100a (no GPU needed: cross-compiles).
+"""In-tree build of libspearmint_b200.so with nvcc for sm_90a (no GPU needed: cross-compiles).
 
     python -m spearmint_b200.build [--force] [--verbose]
 
 The library has no torch / Python dependency; the Python host binds it with ctypes
-(spearmint_b200/_lib.py).  Objects and the .so are git-ignored but travel with gpurun snapshots.
+(spearmint_b200/_lib.py).  Objects and the .so are build products (git-ignored).
 """
 import hashlib
 import os
@@ -17,7 +17,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libspearmint_b200.so")
 SOURCES = ["cov.cu", "potrf.cu", "potrf_ll.cu", "solve.cu", "predict.cu", "predict_tc.cu", "kxt_tc.cu", "guard.cu", "sobol.cu", "ei.cu", "grad.cu", "api.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 
@@ -82,7 +82,7 @@ def _build_locked(force, verbose, stamp, dig):
     with open(os.path.join(LIBDIR, "ptxas.log"), "w") as fh:
         fh.write(log)
     tmp = LIB + ".tmp.%d" % os.getpid()
-    cmd = [NVCC, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [NVCC, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

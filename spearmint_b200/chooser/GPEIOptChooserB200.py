@@ -7,7 +7,7 @@ optional ``obj.generate_stats_html()``.  Same option names and string casts, sam
 same use of the process-global numpy RNG in the same order, same exceptions (LinAlgError, slice-sampler errors).
 
 What changed is where the arithmetic runs: every covariance build, Cholesky, triangular solve, prediction and EI
-evaluation is a hand-written sm_100a kernel behind the C ABI (``spearmint_b200.backend.DeviceBackend``):
+evaluation is a hand-written sm_90a kernel behind the C ABI (``spearmint_b200.backend.DeviceBackend``):
   * hyper-parameter chain  : host slice sampler (util.py), log-likelihood on the GPU in float64      [f2]
   * EI over the grid       : all S samples batched in one pass in float32 (``ei_over_hypers``)        [a1-a10]
   * L-BFGS-B refinement    : scipy on the host, (f, g) from the GPU with the S factors cached         [f1]

@@ -404,7 +404,7 @@ int smk_ei_over_hypers_host_f32(int kind, int N, int M, int D, int S, const doub
   if ((rc = smk_potrf_lower_batched_f32(Npad, S, fac, winv, info, st))) return rc;
   // Factors of fewer than SMK_TC_MIN_N (default 2048) observations take the blocked-substitution chain (3-8x more accurate
   // on the smooth, ill-conditioned problems small N goes with; DESIGN.md section 6), larger ones the tensor-core chain:
-  // explicit inverse (split), alpha by two mat-vecs, fp16 operand pack, tcgen05 3xFP16 predict.
+  // explicit inverse (split), alpha by two mat-vecs, fp16 operand pack, wgmma 3xFP16 predict.
   int tc_min_n = 2048;
   { const char* e = getenv("SMK_TC_MIN_N"); if (e && e[0]) tc_min_n = atoi(e); }
   if (N < tc_min_n) {

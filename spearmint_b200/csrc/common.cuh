@@ -1,4 +1,4 @@
-// common.cuh -- shared device machinery for libspearmint_b200 (sm_100a).
+// common.cuh -- shared device machinery for libspearmint_b200 (sm_90a).
 //
 // The SIMT data path is one register-tiled block GEMM (TileGemm) reused by the Cholesky
 // panel/trailing updates, the multi-RHS triangular solves and the fused predict kernel.
@@ -221,6 +221,11 @@ __device__ __forceinline__ float tf32_rn(float x) {
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
   return __uint_as_float(u);
 }
+// lo part of a split whose ONLY use is as a tf32 tensor-core operand: rounded to tf32 as well.  The MMA reads just the
+// top 10 mantissa bits of an operand, so the unrounded x - tf32_rn(x) would be truncated toward zero -- a bias that
+// accumulates along k through the Cholesky update and the triangular inverse.  (A split that is also read as a float32
+// value, hi + lo, keeps the exact lo.)
+__device__ __forceinline__ float tf32_lo(float x, float hi) { return tf32_rn(x - hi); }
 
 // launch bookkeeping (api.cu)
 void count_launch(int n = 1);

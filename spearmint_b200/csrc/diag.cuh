@@ -2,11 +2,10 @@
 //
 // Reference: spla.cholesky at OPT:540, 567, 585 and inside every slice-sampler log-probability OPT:637, 659, 690.  A
 // blocked factorisation runs Npad / NB diagonal-block steps strictly one after the other, so the latency of one step --
-// not its flops -- bounds the factorisation of a single matrix.  Round 1 did everything a step needs in one kernel with
-// block-wide barriers around every column of every 32 x 32 piece (155 us per 128 x 128 float block, 62 us per 64 x 64
-// double block).  A clock64() timeline of the first rewrite (tools/microbench/diag_bench.cu, profiles/r02_diag_timeline.md)
-// showed where a step really goes -- 33 % assembling the off-diagonal tiles of W = L^-1, 23 % a latency-bound load loop,
-// 20 % the four 32 x 32 factorisations, 12 % the rank-32 updates -- hence this split:
+// not its flops -- bounds the factorisation of a single matrix.  A first version did everything a step needs in one
+// kernel with block-wide barriers around every column of every 32 x 32 piece; a clock64() timeline of it
+// (tools/microbench/diag_bench.cu) showed most of a step going to assembling the off-diagonal tiles of W = L^-1 and to a
+// latency-bound load loop rather than to the 32 x 32 factorisations and rank-32 updates -- hence this split:
 //
 //   diag_factor_block   (one CTA per matrix, ON the spine)  load (8 loads in flight per thread) -> for each 32-piece:
 //                       warp-synchronous Cholesky of the piece (lane = row, row in registers), substitution for the rows
@@ -126,9 +125,9 @@ __device__ __forceinline__ float vget(const float4& v, int i) { return i == 0 ? 
 //
 // What bounds it is the chain  pivot -> rsqrt -> scale -> (column to the other lanes) -> update -> next pivot, once per
 // column, and -- the whole piece being straight-line code that runs once -- the instruction stream itself
-// (tools/microbench/chol32_bench.cu, profiles/r02_diag_timeline.md):
+// (tools/microbench/chol32_bench.cu measures it):
 //   * the next pivot  r[j+1] - l^2  needs no other lane's data: lane j+1 forms it from its own l, so the broadcast of the
-//     column is off the chain (183 cycles per column in float64 against 267, 140 against 252 in float32);
+//     column is off the chain;
 //   * the column is broadcast through shared memory with 16-byte loads instead of one shuffle per element: 3.5 k
 //     instructions per piece instead of 9.7 k (float64), and the function is NOT inlined -- one copy for all call sites,
 //     because the first execution of every further copy cost ~10 k cycles of instruction fetch.
@@ -413,7 +412,7 @@ __device__ void diag_factor_block(T* __restrict__ Ab, int ld, T* __restrict__ wd
 // ------------------------------------------------------------------------------------------------ panel by block substitution
 // 32 rows of the panel below block (jb, jb):  X = A L_jj^-T  as  X_p = (A_p - sum_{q<p} X_q L_pq^T) W_pp^T, p = 0..NP-1.
 // Ap: first of the 32 rows (row stride ld), columns of block column jb;  Ljj: the factored diagonal block (row stride ld);
-// wd: its diagonal inverses.  Result overwrites Ap; optional tf32 (hi, lo) copies for the tcgen05 update (float only).
+// wd: its diagonal inverses.  Result overwrites Ap; optional tf32 (hi, lo) copies for the tensor-core update (float only).
 template <typename T, int NB>
 struct PanelSmem {
   static constexpr int SB = 32, LDT = TileLd<T>::v, NP = NB / SB, TILE = SB * LDT;
@@ -433,7 +432,7 @@ __device__ void panel_sub_block(T* __restrict__ Ap, int ld, const T* __restrict_
   T* tt = xt + NP * TILE;                   // scratch: A_p - sum
   const int tid = threadIdx.x;
   // ---- loads: every thread issues all of its global reads before the first shared-memory store (this kernel sits on the
-  //      spine: a load loop with one request in flight per thread cost 17 of its 20 us)
+  //      spine: a load loop with one request in flight per thread is latency-bound)
   {
     constexpr int NLV = PS::NL * 4, NWV = NP * 4, NXV = NB / 8;       // values per thread: L tiles, W tiles, panel rows
     T lv[NLV > 0 ? NLV : 1], wv[NWV], xv[NXV];
@@ -510,7 +509,7 @@ __device__ void panel_sub_block(T* __restrict__ Ap, int ld, const T* __restrict_
       if (hi != nullptr) {                   // tf32 (hi, lo) copy of the finished panel: round-to-nearest split
         const float h = tf32_rn(x);
         hi[(long)i * ld + k] = h;
-        lo[(long)i * ld + k] = x - h;
+        lo[(long)i * ld + k] = tf32_lo(x, h);
       }
     }
   }

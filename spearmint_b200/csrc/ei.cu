@@ -26,7 +26,7 @@ __device__ __forceinline__ double ei_one(double best, double m, double v) {
 // u Phi(u) + phi(u) cancels by less than a factor 20 and erfcf / expf keep the result within ~5e-6 relative of the double
 // value (the moments themselves carry 1e-4) -- and in double in the tail, where the chooser ranks candidates by values
 // that float32 would flush to zero.  This is what makes the sweep an HBM sweep (12-16 bytes per pair against ~45
-// float32 instructions) instead of an fp64-ALU loop (profiles/r02_ei_sweep_bandwidth.md).  The result is a double either way.
+// float32 instructions) instead of an fp64-ALU loop.  The result is a double either way.
 __device__ __forceinline__ double ei_one(double best, float m, float v) { return ei_one(best, (double)m, (double)v); }
 __device__ __forceinline__ double ei_one_f32(float best, float m, float v) {
   if (v > 0.f) {

@@ -1,10 +1,10 @@
 // guard.cu -- accuracy guard of the tensor-core predict path.
 //
-// The tcgen05 predict forms beta = Linv * kx with an EXPLICIT float32 inverse of the Cholesky factor.  That is not
+// The tensor-core predict forms beta = Linv * kx with an EXPLICIT float32 inverse of the Cholesky factor.  That is not
 // backward stable: the variance  amp2 (1 + 1e-6) - |beta|^2  of a candidate close to the data carries an error of about
 // eps32 * ||K||_2 * |K^-1 kx|^2, which for smooth low-dimensional problems (D = 8, N = 512: ||K|| ~ 340, noise 1e-3)
 // is percents of the variance itself -- above the stated 5e-3 EI tolerance -- while the blocked substitution of the
-// SIMT predict kernel stays within it (tools/tc_error_probe.py, profiles/r02_precision_guard.md).
+// SIMT predict kernel stays within it (tools/tc_error_probe.py).
 //
 // The guard measures exactly that error, on the device, before any candidate is touched.  For a few observed points
 // x_i (the caller passes the incumbents -- the lowest observed values, where EI concentrates and where the chooser's own
@@ -53,11 +53,10 @@ __global__ void __launch_bounds__(256) guard_lv_kernel(int N, int Npad, int Np, 
 
 // acc[s][q]      += sum over this block's rows r of b_r^2,           b_r = sum_{j <= r} Linv[r][j] p[q][j]
 // acc[s][Q + q]  += sum over this block's rows r of 2 b_r t_r,       t_r = the accumulation bias of the tensor-core GEMM:
-//   tcgen05 accumulates in float32 with truncation; along a row of L^-1 the running sum is negative almost to the end (the
+//   the tensor core accumulates in float32 with truncation; along a row of L^-1 the running sum is negative almost to the end (the
 //   off-diagonal entries of the inverse of a positive matrix are mostly negative, the diagonal -- the LAST term -- is large
 //   and positive), so every one of the 3 MMAs per 16 observations loses about half an ulp of the running sum in the same
-//   direction:  t_r = -3 * 2^-24 * sum over 16-wide steps of the running sum  (measured: tools/tc_error_probe.py,
-//   profiles/r02_precision_guard.md).
+//   direction:  t_r = -3 * 2^-24 * sum over 16-wide steps of the running sum  (tools/tc_error_probe.py measures it).
 __global__ void __launch_bounds__(256) guard_bv_kernel(int N, int Np, const float* __restrict__ hi, const float* __restrict__ lo,
                                                         const double* __restrict__ p, double* __restrict__ acc) {
   const int s = blockIdx.y, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;

@@ -8,31 +8,23 @@
 // SAMPLE) on  r2_s = sum_d ((x_d - c_d) / ls_sd)^2  and is bound by the float32 pipe.  But
 //     r2_s(c, n) = sum_d  w_sd * q_d(c, n),      q_d = (x_nd - c_cd)^2   (sample independent),  w_sd = 1 / ls_sd^2
 // is a GEMM over d:  q is formed ONCE per (pair, dimension) on the CUDA cores -- in the difference form, so nothing
-// cancels, and every term of the sum is non-negative -- and the contraction for all S samples runs on tcgen05 as
+// cancels, and every term of the sum is non-negative -- and the contraction for all S samples runs on wgmma as
 // 3 x FP16 products with exact power-of-two operand scaling (the scheme of the predict GEMM; DESIGN.md 6).
 //
-// Mapping (chosen for the epilogue, which is where the time goes):  accumulator row (TMEM lane) = (candidate slot j,
-// sample s), column = observation n.  J = min(128 / S, 96 / Dp) candidates share the 128 lanes through a block-diagonal
-// A operand: row (j, s) holds w_s in k-block j and zeros elsewhere; the B operand row of observation n is
-// [q(c_0, n) | ... | q(c_J-1, n)].  So each epilogue thread owns ONE sample of ONE candidate and walks along n:
-// per-thread sample constants, float4 loads of alpha_s[n..], 16-byte stores of 8 consecutive halves, and the mean is a
-// private running sum -- no cross-lane reduction anywhere.  (A first version with lane = observation needed 2-byte
-// stores, 40 samples of state per thread and a transposing butterfly: 80 ms vs 64 ms for the SIMT kernel.)
+// Mapping (chosen for the epilogue, which is where the time goes):  accumulator row = (candidate slot j, sample s),
+// column = observation n.  J = min(128 / S, 96 / Dp) candidates share the 128 rows through a block-diagonal A operand:
+// row (j, s) holds w_s in k-block j and zeros elsewhere; the B operand row of observation n is [q(c_0, n) | ... |
+// q(c_J-1, n)].  The per-row constants (sample scale, amplitude) are fixed per thread, and the predictive mean is a
+// running sum per row.
 //
-// STATUS (round 1): numerically complete and parity-tested against the float64 oracle (tests/test_gpu_kernels.py::
-// test_kxt_generators_match_oracle); 56-59 ms per headline step against 63-64 ms for the packed-float32 SIMT generator
-// (same box).  With lane = (candidate, sample) a naive epilogue issues 16-byte global accesses that are 32 separate sectors
-// per warp instruction; that version ran at 146 ms with every warp 8-10x slower than its instruction stream (clock64
-// timeline + ncu: profiles/r01_kxt_tc_ncu.md).  Hence the output chunk is transposed through shared memory before it is
-// stored (8 x 64-byte segments per store instruction), alpha is staged per 32-column chunk with coalesced reads, and the
-// observations are read dimension-major.  Opt-in (SMK_KXT_IMPL=tc) until it has been through a full verification round as
-// the default; predict_tc() uses the SIMT generator otherwise, and always for D > 32 or when the shared-memory budget of
-// this kernel does not fit the sample count.
-//
-// Roles in a CTA of 17 warps:  warps 0-3 producers (thread = observation row: q for the J candidate slots -> fp16 (hi, lo)
-// -> shared memory in the 64-byte-swizzled K-major layout, one [128 x 64 B] block per candidate slot; warp 3 owns the TMEM
-// allocation);  warps 4-15 three epilogue groups (tile t -> group t mod 3), 4 TMEM buffers of 128 columns;  warp 16: lane 0
-// issues the MMAs of every tile.  Work item = J candidates x all observations.
+// A CTA is two warpgroups; warpgroup g owns accumulator rows 64 g .. 64 g + 63 (wgmma m64n128k16, 3 x FP16 products per
+// k step, accumulator in registers).  Work item = J candidates x all observations, in tiles of 128 observations.  All 256
+// threads build the q operand of tile t + 1 (fp16 hi, lo in the 64-byte-swizzled K-major layout, one [128 x 64 B] block
+// per candidate slot) while the MMAs of tile t run, then turn the accumulator of tile t into kernel values.  Each warp
+// transposes its 16 rows x 128 columns of output through shared memory, so that every store instruction writes one
+// 256-byte row of hi and one of lo.  Opt-in (SMK_KXT_IMPL=tc): on an H100 SXM it is slower than the SIMT generator at the
+// headline shape (95 against 80 ms per step); predict_tc() uses the SIMT generator otherwise, and always for D > 32 or
+// where kxt_tc_preferred() says few samples would leave most accumulator rows empty.
 #include <cuda_fp16.h>
 #include <cuda.h>
 
@@ -50,19 +42,14 @@ int num_sms();
 namespace ktc {
 using namespace tc;
 
-constexpr int TN = 128;            // observations per tile (MMA N, TMEM columns per buffer)
-constexpr int BSTAGES = 2;         // B-operand (q tile) stages
-constexpr int TBUF = 4;            // TMEM accumulator buffers (4 x 128 columns)
-constexpr int NGRP = 3;            // epilogue groups
+constexpr int TN = 128;            // observations per tile (MMA N)
 constexpr int MAXD = 32;           // padded dimension limit
-constexpr int MAXK = 96;           // J * Dp limit: one q stage = 128 x 96 halves x (hi, lo) = 48 KB
-constexpr int MAXS = 64;           // samples per launch (one sample per TMEM lane: <= 128; the alpha prefetch holds MAXS / 16 float4 per thread)
-constexpr int THREADS = 17 * 32;     // 4 producer warps, 12 epilogue warps, 1 MMA-issue warp
-constexpr int CW = 32;             // columns per epilogue chunk (one tcgen05.ld.x32)
-constexpr int ALD = CW + 4;        // row length (floats) of the staged alpha chunk: 144-byte stride -> conflict-free row reads
-constexpr int OLD = 144;           // bytes per row of the output staging: 64 B hi | 64 B lo | 16 B pad (conflict-free both ways)
-constexpr int GRP_OUT = 4 * 32 * OLD;            // output staging of one group (one [32 rows] block per warp)
-constexpr int GRP_BASE = 128 * 8;                // per-row global element offsets of the current item
+constexpr int MAXK = 96;           // J * Dp limit: one q buffer = 128 x 96 halves x (hi, lo) = 48 KB
+constexpr int MAXS = 64;           // samples per launch (one sample per accumulator row: <= 128)
+constexpr int THREADS = 256;       // two warpgroups
+constexpr int NGRP = 1;            // mean partial planes per chunk
+constexpr int OLDH = TN + 8;       // halves per row of the output staging: 272-byte stride, conflict-free fragment stores
+constexpr int WARP_STG = 2 * 16 * OLDH;           // halves of one warp's staging: hi rows 0-15, then lo rows 0-15
 
 struct Args {
   int kind, N, Np, M, c_begin, Mc, D, Dp, S, J, K, Npad_alpha;
@@ -73,127 +60,48 @@ struct Args {
   const unsigned* qmax;            // [2] float bits of max|X|, max|C|
   __half *khi, *klo;               // [S][Mc][Np]
   float* mu_partial;               // [NGRP][S][Mc]
-  long long* tl;                   // optional timeline (SMK_KXT_TIMELINE=1): [tile < 64][8] clock64() stamps of CTA 0
+  long long* tl;                   // optional timeline (SMK_KXT_TIMELINE=1): [tile < 64][8] clock64() stamps of CTA 0 (slots 0-3 used)
 };
 constexpr int TL_TILES = 64;
 __device__ long long g_timeline[TL_TILES * 8];
 
 __host__ __device__ inline int slots(int S, int Dp) { int j = 128 / S, k = MAXK / Dp; return j < k ? j : k; }
 
-__host__ __device__ inline size_t smem_bytes(int K, int S) {
-  return (size_t)BSTAGES * 2 * TN * K * 2 + (size_t)2 * 128 * K * 2 + MAXK * 4 /*candidate rows*/ +
-         (size_t)NGRP * ((size_t)S * ALD * 4 /*alpha chunk*/ + GRP_OUT + GRP_BASE) + 256 /*barriers*/ + 1024 /*align*/;
+__host__ __device__ inline size_t smem_bytes(int K, int /*S*/) {
+  return (size_t)2 * 128 * K * 2 /*A hi, lo*/ + (size_t)2 * 2 * TN * K * 2 /*two q buffers*/ +
+         (size_t)(THREADS / 32) * WARP_STG * 2 /*output staging*/ + 1024 /*align*/;
 }
 
 // Operand tiles are K-major with the 64-byte swizzle (one candidate slot = 32 halves = one 64-byte row), stored as
-// J blocks of [128 rows x 64 B]; the 16-byte chunk c of row r sits at chunk (c ^ ((r >> 1) & 3)) -- Swizzle<2,4,3> on
-// byte addresses, the pattern TMA produces for CU_TENSOR_MAP_SWIZZLE_64B and tcgen05.mma expects for layout type 4.
-// (A first version used the no-swizzle core-matrix layout: numerically fine, but each 128x128x16 MMA then took ~1600
-// cycles -- the tensor pipe was 4.9 % active while every other warp waited for it; ncu, profiles/r01_kxt_tc_ncu.md.)
+// J blocks of [128 rows x 64 B]; the 16-byte chunk c of row r sits at chunk (c ^ ((r >> 1) & 3)) -- the pattern TMA
+// produces for CU_TENSOR_MAP_SWIZZLE_64B and wgmma expects for a 64-byte-swizzle descriptor.
 constexpr uint32_t SLOT_BYTES = 128 * 64;
-__device__ __forceinline__ uint32_t core_off(int r, int jbg, int /*C*/) {
+__device__ __forceinline__ uint32_t core_off(int r, int jbg) {
   return (uint32_t)(jbg >> 2) * SLOT_BYTES + (uint32_t)r * 64u + (uint32_t)(((jbg & 3) ^ ((r >> 1) & 3)) << 4);
-}
-__device__ __forceinline__ uint64_t desc_sw64(uint32_t saddr) {
-  uint64_t d = (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;                                  // leading byte offset (ignored for swizzled K-major)
-  d |= (uint64_t)(512 >> 4) << 32;                         // stride byte offset: 8 rows x 64 B
-  d |= (uint64_t)1 << 46;                                  // descriptor version (Blackwell)
-  d |= (uint64_t)4 << 61;                                  // SWIZZLE_64B
-  return d;
-}
-
-// kind::f16, f16 x f16 -> f32, both operands K-major, M = 128, N = 128
-constexpr uint32_t kIdesc = (1u << 4) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(kIdesc), "r"(accumulate)
-      : "memory");
 }
 
 __device__ __forceinline__ unsigned h2_bits(__half2 h) { return *reinterpret_cast<unsigned*>(&h); }
 
-// One 32-column chunk of one accumulator row: distances -> kernel values -> scaled fp16 (hi, lo) into this lane's staging row,
-// running mean.  KIND and EDGE are compile-time: the per-pair kind switch and edge test were ~20 % of the executed instructions.
-template <int KIND, bool EDGE, bool MU>
-__device__ __forceinline__ void chunk_compute(const uint32_t (&r)[32], float2 scl2, float2 a2s, const float* al_row,
-                                              unsigned char* gout_row, int nfirst, int N, float2& v) {
-#pragma unroll
-  for (int k8 = 0; k8 < 4; ++k8) {             // 8 columns -> 16 bytes of hi and of lo in this lane's staging row
-    unsigned ph[4], pl[4];
-    float2 ap[4];
-    if (MU) {
-      const float4 a0 = *reinterpret_cast<const float4*>(al_row + 8 * k8);
-      const float4 a1 = *reinterpret_cast<const float4*>(al_row + 8 * k8 + 4);
-      ap[0] = make_float2(a0.x, a0.y); ap[1] = make_float2(a0.z, a0.w); ap[2] = make_float2(a1.x, a1.y); ap[3] = make_float2(a1.z, a1.w);
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int col = 8 * k8 + 2 * i;
-      float2 r2 = __fmul2_rn(make_float2(__uint_as_float(r[col]), __uint_as_float(r[col + 1])), scl2);
-      r2.x = fmaxf(r2.x, 0.f);                 // the (hi, lo) products can leave -1 ulp at coincident points
-      r2.y = fmaxf(r2.y, 0.f);
-      float2 kk = kernel_pair_fast_t<KIND>(r2);
-      if (EDGE) {                              // padded observations carry no covariance
-        const int n = nfirst + col;
-        if (n >= N) kk.x = 0.f;
-        if (n + 1 >= N) kk.y = 0.f;
-      }
-      if (MU) v = __ffma2_rn(kk, ap[i], v);
-      const float2 val = __fmul2_rn(kk, a2s);
-      const __half2 h2 = __floats2half2_rn(val.x, val.y);
-      const float2 hf = __half22float2(h2);
-      const __half2 l2 = __floats2half2_rn(val.x - hf.x, val.y - hf.y);
-      ph[i] = h2_bits(h2);
-      pl[i] = h2_bits(l2);
-    }
-    *reinterpret_cast<uint4*>(gout_row + k8 * 16) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
-    *reinterpret_cast<uint4*>(gout_row + 64 + k8 * 16) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
-  }
-}
-
 template <int KIND, bool MU>
 __global__ void __launch_bounds__(THREADS, 1) kxt_tc_kernel(Args p) {
   extern __shared__ unsigned char smem_raw[];
-  // 1 KB alignment by OFFSET, not by integer arithmetic on the pointer: a pointer rebuilt from a uintptr_t loses its address
-  // space, and every shared-memory access of the kernel became a generic LD.E / ST.E on the long scoreboard (ncu r02:
-  // 38 % of all stall samples were long-scoreboard waits on what should have been LDS / STS).
+  // 1 KB alignment by OFFSET, not by integer arithmetic on the pointer: a pointer rebuilt from a uintptr_t loses its
+  // address space, and every shared-memory access would become a generic one.
   unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int Dp = p.Dp, K = p.K, C = K >> 3, CD = Dp >> 3;   // 16-byte k blocks per operand row / per candidate slot (4)
   const uint32_t BH = (uint32_t)TN * K * 2;          // bytes of one B half (hi or lo)
   const uint32_t WH = (uint32_t)128 * K * 2;
-  unsigned char* sB = base;
-  unsigned char* sW = sB + (size_t)BSTAGES * 2 * BH;
-  float* cs = reinterpret_cast<float*>(sW + 2 * WH);             // [J][Dp] candidate rows of the current item
-  unsigned char* sGrp = reinterpret_cast<unsigned char*>(cs + MAXK);   // per epilogue group: alpha chunk | output staging | row offsets
-  const size_t grp_bytes = (size_t)p.S * ALD * 4 + GRP_OUT + GRP_BASE;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sGrp + NGRP * grp_bytes);
-  uint64_t* b_full = bars;
-  uint64_t* b_empty = b_full + BSTAGES;
-  uint64_t* t_full = b_empty + BSTAGES;
-  uint64_t* t_empty = t_full + TBUF;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(t_empty + TBUF);
+  unsigned char* sW = base;
+  unsigned char* sB = sW + 2 * WH;                   // [2 buffers][hi | lo]
+  __half* stg = reinterpret_cast<__half*>(sB + 4 * BH);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   // operand scale of q = (x - c)^2: even exponent, half of it is already applied to the coordinates (kxt_prep_kernel)
   const float xmax = __uint_as_float(p.qmax[0]) + __uint_as_float(p.qmax[1]);
   const int eq = scale_exp(xmax * xmax) & ~1;
 
-  if (tid == 0) {
-    for (int i = 0; i < BSTAGES; ++i) { mbar_init(&b_full[i], 4); mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < TBUF; ++i) { mbar_init(&t_full[i], 1); mbar_init(&t_empty[i], 4); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 3) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   // A operand: row (j, s) = w_s * 2^ew_s in k-block j, zero elsewhere (and zero rows beyond J * S); fp16 (hi, lo)
-  for (int e = tid; e < 128 * (K >> 3); e += THREADS) {       // one 16-byte block (8 dimensions) per iteration
+  for (int e = tid; e < 128 * C; e += THREADS) {     // one 16-byte block (8 dimensions) per iteration
     const int r = e / C, jb = e % C;
     const int j = r / p.S, s = r - j * p.S;
     __half2 hh[4], ll[4];
@@ -218,230 +126,158 @@ __global__ void __launch_bounds__(THREADS, 1) kxt_tc_kernel(Args p) {
         ll[k] = __floats2half2_rn(w[0] - hf.x, w[1] - hf.y);
       }
     }
-    const uint32_t off = core_off(r, jb, C);
+    const uint32_t off = core_off(r, jb);
     *reinterpret_cast<uint4*>(sW + off) = make_uint4(h2_bits(hh[0]), h2_bits(hh[1]), h2_bits(hh[2]), h2_bits(hh[3]));
     *reinterpret_cast<uint4*>(sW + WH + off) = make_uint4(h2_bits(ll[0]), h2_bits(ll[1]), h2_bits(ll[2]), h2_bits(ll[3]));
   }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
   const int nblocks = p.Np / TN;
+  // q operand of tile t (item blockIdx.x + (t / nblocks) * gridDim.x, observations of block t % nblocks) into buffer buf.
+  // Thread = observation row (tid % 128) and every other 8-dimension block of the item's candidate slots; Xp is stored
+  // dimension-major ([Dp][Np]), so a warp reads 128 contiguous bytes per dimension.
+  auto build = [&](long t, int buf) {
+    const long item = blockIdx.x + (t / nblocks) * gridDim.x;
+    const int nb = (int)(t % nblocks);
+    const int c0 = p.c_begin + (int)item * p.J;     // first candidate of the item (rows of Cp beyond M are clamped copies)
+    const int r = tid & 127;
+    unsigned char* bh = sB + (size_t)buf * 2 * BH;
+    unsigned char* bl = bh + BH;
+    const float* xcol = p.Xp + (size_t)nb * TN + r;
+    for (int jbg = tid >> 7; jbg < p.J * CD; jbg += 2) {
+      const int j = jbg / CD, jb = jbg - j * CD;
+      const float4* crow = reinterpret_cast<const float4*>(p.Cp + (size_t)(c0 + j) * Dp + 8 * jb);
+      const float4 c0v = __ldg(crow), c1v = __ldg(crow + 1);
+      const float cc[8] = {c0v.x, c0v.y, c0v.z, c0v.w, c1v.x, c1v.y, c1v.z, c1v.w};
+      __half2 hh[4], ll[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float2 xx = make_float2(__ldg(xcol + (size_t)(8 * jb + 2 * k) * p.Np), __ldg(xcol + (size_t)(8 * jb + 2 * k + 1) * p.Np));
+        const float2 df = fadd2(xx, make_float2(-cc[2 * k], -cc[2 * k + 1]));
+        const float2 q = fmul2(df, df);
+        hh[k] = __floats2half2_rn(q.x, q.y);
+        const float2 hf = __half22float2(hh[k]);
+        ll[k] = __floats2half2_rn(q.x - hf.x, q.y - hf.y);
+      }
+      const uint32_t off = core_off(r, jbg);
+      *reinterpret_cast<uint4*>(bh + off) = make_uint4(h2_bits(hh[0]), h2_bits(hh[1]), h2_bits(hh[2]), h2_bits(hh[3]));
+      *reinterpret_cast<uint4*>(bl + off) = make_uint4(h2_bits(ll[0]), h2_bits(ll[1]), h2_bits(ll[2]), h2_bits(ll[3]));
+    }
+  };
 
-  if (warp < 4) {
-    // ------------------------------------------------------------------------------------- producers (+ MMA issue)
-    // thread = observation row of the tile.  Its coordinates come as 8 independent float4 loads, prefetched one tile
-    // ahead (a first version with serial rounds of dependent loads per (row, slot) unit was latency-bound: 21 us per
-    // tile); the J candidate rows of the item sit in shared memory.  Lane 0 of warp 3 also issues the MMAs of the tile.
-    const int r = tid;
-    const uint64_t whi = desc_sw64(smem_u32(sW)), wlo = desc_sw64(smem_u32(sW + WH));
-    const int ksteps = K / 16;
-    // Xp is stored dimension-major ([Dp][Np]): the 32 lanes of a warp read 128 contiguous bytes per dimension
-    float xc[MAXD], xn[MAXD];
+  // this thread's accumulator rows r0 and r0 + 8 (fragment layout: tc_common.cuh) and their per-row constants
+  const int wg = warp >> 2;
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  int rj[2], rs[2];
+  float2 scl2[2], a2s[2];
 #pragma unroll
-    for (int d = 0; d < MAXD; ++d) xc[d] = __ldg(p.Xp + (size_t)d * p.Np + r);
-    long t = 0;
-    for (long item = blockIdx.x; item < p.nitems; item += gridDim.x) {
-      const int c0 = p.c_begin + (int)item * p.J;     // first candidate of the item (rows of Cp beyond M are clamped copies)
-      asm volatile("bar.sync 1, 128;" ::: "memory");  // every producer is done with the previous item's candidate rows
-      for (int e = tid; e < K / 4; e += 128)
-        reinterpret_cast<float4*>(cs)[e] = __ldg(reinterpret_cast<const float4*>(p.Cp + (size_t)c0 * Dp) + e);
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      for (int nb = 0; nb < nblocks; ++nb, ++t) {
-        const int nbn = (nb + 1 == nblocks) ? 0 : nb + 1;
-#pragma unroll
-        for (int d = 0; d < MAXD; ++d) xn[d] = __ldg(p.Xp + (size_t)d * p.Np + nbn * TN + r);
-        const int st = (int)(t % BSTAGES);
-        mbar_wait_relaxed(&b_empty[st], (uint32_t)(((t / BSTAGES) & 1) ^ 1), 128);
-        const bool stamp = p.tl && blockIdx.x == 0 && t < TL_TILES;
-        if (stamp && tid == 0) p.tl[t * 8 + 0] = clock64();
-        unsigned char* bh = sB + (size_t)st * 2 * BH;
-        unsigned char* bl = bh + BH;
-        for (int j = 0; j < p.J; ++j) {
-#pragma unroll
-          for (int jb = 0; jb < MAXD / 8; ++jb) {
-            if (jb < CD) {
-              const float4 c0v = *reinterpret_cast<const float4*>(&cs[j * Dp + 8 * jb]);
-              const float4 c1v = *reinterpret_cast<const float4*>(&cs[j * Dp + 8 * jb + 4]);
-              const float2 xx[4] = {make_float2(xc[8 * jb], xc[8 * jb + 1]), make_float2(xc[8 * jb + 2], xc[8 * jb + 3]),
-                                    make_float2(xc[8 * jb + 4], xc[8 * jb + 5]), make_float2(xc[8 * jb + 6], xc[8 * jb + 7])};
-              const float2 cc[4] = {make_float2(-c0v.x, -c0v.y), make_float2(-c0v.z, -c0v.w), make_float2(-c1v.x, -c1v.y),
-                                    make_float2(-c1v.z, -c1v.w)};
-              __half2 hh[4], ll[4];
-#pragma unroll
-              for (int k = 0; k < 4; ++k) {
-                const float2 df = __fadd2_rn(xx[k], cc[k]);
-                const float2 q = __fmul2_rn(df, df);
-                hh[k] = __floats2half2_rn(q.x, q.y);
-                const float2 hf = __half22float2(hh[k]);
-                ll[k] = __floats2half2_rn(q.x - hf.x, q.y - hf.y);
-              }
-              const uint32_t off = core_off(r, j * CD + jb, C);
-              *reinterpret_cast<uint4*>(bh + off) = make_uint4(h2_bits(hh[0]), h2_bits(hh[1]), h2_bits(hh[2]), h2_bits(hh[3]));
-              *reinterpret_cast<uint4*>(bl + off) = make_uint4(h2_bits(ll[0]), h2_bits(ll[1]), h2_bits(ll[2]), h2_bits(ll[3]));
-            }
-          }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to tcgen05.mma
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&b_full[st]);
-        if (stamp && tid == 0) p.tl[t * 8 + 1] = clock64();
-        __syncwarp();
-#pragma unroll
-        for (int d = 0; d < MAXD; ++d) xc[d] = xn[d];
-      }
-    }
-  } else if (warp == 16) {
-    // ------------------------------------------------------------------------------------------------ MMA issue
-    // Its own warp: when lane 0 of a producer warp issued the MMAs, that warp could not start the next tile before the
-    // other three had delivered this one and a TMEM buffer was free -- the slowest producer set the pace, and its
-    // single-lane spin (4.8e8 loop iterations per launch, a quarter of all executed instructions in the r02 profile) sat
-    // in the producers' own issue slots.
-    if (lane == 0) {
-      const uint64_t whi = desc_sw64(smem_u32(sW)), wlo = desc_sw64(smem_u32(sW + WH));
-      const int ksteps = K / 16;
-      long t = 0;
-      for (long item = blockIdx.x; item < p.nitems; item += gridDim.x) {
-        for (int nb = 0; nb < nblocks; ++nb, ++t) {
-          const int st = (int)(t % BSTAGES), b = (int)(t % TBUF);
-          const bool stamp = p.tl && blockIdx.x == 0 && t < TL_TILES;
-          if (stamp) p.tl[t * 8 + 2] = clock64();
-          mbar_wait_relaxed(&t_empty[b], (uint32_t)(((t / TBUF) & 1) ^ 1), 32);
-          mbar_wait_relaxed(&b_full[st], (uint32_t)((t / BSTAGES) & 1), 32);
-          if (stamp) p.tl[t * 8 + 3] = clock64();
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t d = tmem_base + (uint32_t)b * TN;
-          const uint32_t sb = smem_u32(sB + (size_t)st * 2 * BH);
-          const uint64_t bhi = desc_sw64(sb), blo = desc_sw64(sb + BH);
-          for (int q = 0; q < ksteps; ++q) {
-            const uint64_t ko = (uint64_t)(((q >> 1) * SLOT_BYTES + (q & 1) * 32) >> 4);   // slot block, then 32 B inside the row
-            umma_f16(d, wlo + ko, bhi + ko, q ? 1u : 0u);              // small terms first
-            umma_f16(d, whi + ko, blo + ko, 1u);
-            umma_f16(d, whi + ko, bhi + ko, 1u);
-          }
-          umma_commit(&b_empty[st]);
-          umma_commit(&t_full[b]);
-          if (stamp) p.tl[t * 8 + 4] = clock64();
-        }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------------------------------------ epilogue
-    const int grp = (warp - 4) >> 2;                  // tiles t with t mod 3 == grp
-    const int q4 = warp & 3;                          // TMEM lane quarter this warp may read
-    const int L = q4 * 32 + lane;                     // accumulator row = (candidate slot, sample)
-    const int j = L / p.S, s = L - j * p.S;
-    const bool row_used = j < p.J;
+  for (int rh = 0; rh < 2; ++rh) {
+    const int L = r0 + 8 * rh;
+    rj[rh] = L / p.S;
+    rs[rh] = L - rj[rh] * p.S;
     float scl = 0.f, a2 = 0.f;
-    if (row_used) {
+    if (rj[rh] < p.J) {
       float wmax = 0.f;
-      for (int d = 0; d < p.D; ++d) { const float il = p.inv_ls[(long)s * p.D + d]; wmax = fmaxf(wmax, il * il); }
+      for (int d = 0; d < p.D; ++d) { const float il = p.inv_ls[(long)rs[rh] * p.D + d]; wmax = fmaxf(wmax, il * il); }
       scl = ldexpf(1.f, -(eq + scale_exp(wmax)));
-      a2 = p.amp2[s];
+      a2 = p.amp2[rs[rh]];
     }
-    const float2 scl2 = dup2(scl);
-    const float2 a2s = dup2(a2 * ldexpf(1.f, kx_exp(a2)));
-    unsigned char* gbase = sGrp + (size_t)grp * grp_bytes;
-    float* gal = reinterpret_cast<float*>(gbase);                                   // alpha chunk [S][ALD]
-    unsigned char* gout = gbase + (size_t)p.S * ALD * 4 + (size_t)q4 * 32 * OLD;    // this warp's output staging [32 rows][OLD]
-    long long* rowoff = reinterpret_cast<long long*>(gbase + (size_t)p.S * ALD * 4 + GRP_OUT);   // [128] element offsets, -1 = no row
-    const float* al_row = gal + (size_t)(row_used ? s : 0) * ALD;
-    const int gt = tid - 128 - grp * 128;             // thread index inside the group (0..127) == accumulator row L
-    const int bar_id = 2 + grp;
-    long t = 0;
-    // alpha_s[n .. n+31] of the chunk starting at observation n, for all samples: this thread's share (coalesced 128-byte
-    // row reads), kept in registers until the group's shared-memory copy may be overwritten.  The loads of chunk c+1 are
-    // issued before chunk c is computed, so their latency never sits between the two barriers of a chunk.
-    constexpr int APF = MAXS * (CW / 4) / 128;          // float4 per thread at the sample limit (4)
-    float4 apf[APF];
-    auto alpha_fetch = [&](int nbase) {
-#pragma unroll
-      for (int q = 0; q < APF; ++q) {
-        const int f = gt + q * 128;
-        if (f < p.S * (CW / 4)) {
-          const int rs = f >> 3, c4 = (f & 7) * 4, n = nbase + c4;
-          const float* src = p.alpha + (size_t)rs * p.Npad_alpha + n;
-          if (n + 3 < p.N) apf[q] = __ldg(reinterpret_cast<const float4*>(src));
-          else apf[q] = make_float4(n < p.N ? src[0] : 0.f, n + 1 < p.N ? src[1] : 0.f, n + 2 < p.N ? src[2] : 0.f, 0.f);
-        }
-      }
-    };
-    auto alpha_store = [&]() {
-#pragma unroll
-      for (int q = 0; q < APF; ++q) {
-        const int f = gt + q * 128;
-        if (f < p.S * (CW / 4)) *reinterpret_cast<float4*>(gal + (size_t)(f >> 3) * ALD + (f & 7) * 4) = apf[q];
-      }
-    };
-    if (MU) {                                            // first chunk of this group: tile nb = grp of the first item
-      const int nb_first = grp % nblocks;
-      alpha_fetch(nb_first * TN);
-    }
-    for (long item = blockIdx.x; item < p.nitems; item += gridDim.x) {
-      const int crow = (int)item * p.J + j;           // candidate row inside the chunk
-      const bool act = row_used && crow < p.mc_used;
-      // the group (MU: alpha chunk shared by its 4 warps) / the warp (rowoff rows are read by their own warp only) is done
-      // with the previous item's offsets
-      if (MU) asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
-      else __syncwarp();
-      rowoff[gt] = act ? (long long)(((size_t)s * p.Mc + crow) * p.Np) : -1;
-      if (!MU) __syncwarp();
-      float2 v = make_float2(0.f, 0.f);
-      for (int nb = 0; nb < nblocks; ++nb, ++t) {
-        if ((int)(t % NGRP) != grp) continue;
-        const int b = (int)(t % TBUF);
-        const int n0 = nb * TN;
-        const bool edge = n0 + TN > p.N;
-        const bool stamp = p.tl && blockIdx.x == 0 && t < TL_TILES && q4 == 0 && lane == 0;
-        if (stamp) p.tl[t * 8 + 5] = clock64();
-        mbar_wait_relaxed(&t_full[b], (uint32_t)((t / TBUF) & 1), 256);
-        if (stamp) p.tl[t * 8 + 6] = clock64();
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t t0 = tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)b * TN;
-#pragma unroll 1
-        for (int cq = 0; cq < TN; cq += CW) {
-          uint32_t r[32];
-          tmem_ld32(t0 + cq, r);
-          if (MU) {
-            asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");        // previous chunk's readers are done
-            alpha_store();                                                       // this chunk's alpha: fetched a chunk ago
-            asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");        // (also publishes rowoff of a new item)
-            // next chunk of this group: same tile, or the group's next tile (t + NGRP; alpha does not depend on the item)
-            alpha_fetch((cq + CW < TN) ? n0 + cq + CW : (int)(((t + NGRP) % nblocks) * TN));
-          }
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if (act) {
-            if (edge) chunk_compute<KIND, true, MU>(r, scl2, a2s, al_row, gout + lane * OLD, n0 + cq, p.N, v);
-            else chunk_compute<KIND, false, MU>(r, scl2, a2s, al_row, gout + lane * OLD, n0 + cq, p.N, v);
-          }
-          __syncwarp();
-          // coalesced write-out: each store instruction covers 4 rows x (64 B hi, 64 B lo); lane -> (row, half, 16-byte piece)
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rho = 4 * i + (lane >> 3), seg = (lane >> 2) & 1, piece = lane & 3;
-            const long long off = rowoff[q4 * 32 + rho];
-            if (off >= 0) {
-              const uint4 dv = *reinterpret_cast<const uint4*>(gout + rho * OLD + seg * 64 + piece * 16);
-              __half* dst = (seg ? p.klo : p.khi) + off + n0 + cq + piece * 8;
-              *reinterpret_cast<uint4*>(dst) = dv;
-            }
-          }
-          __syncwarp();
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&t_empty[b]);
-        if (stamp) p.tl[t * 8 + 7] = clock64();
-      }
-      if (MU && act) p.mu_partial[((size_t)grp * p.S + s) * p.Mc + crow] = v.x + v.y;
-    }
+    scl2[rh] = dup2(scl);
+    a2s[rh] = dup2(a2 * ldexpf(1.f, kx_exp(a2)));
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  __half* wst = stg + (size_t)warp * WARP_STG;
+  const uint32_t a_off = (uint32_t)wg * 64 * 64;      // first row of this warpgroup inside every slot block
+  const int ksteps = K / 16;
+
+  const long my_items = (p.nitems - blockIdx.x + gridDim.x - 1) / gridDim.x;
+  const long T = my_items * nblocks;
+  build(0, 0);
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
   __syncthreads();
-  if (warp == 3) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+  float d[TN / 2];
+  float2 v[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
+  for (long t = 0; t < T; ++t) {
+    const int buf = (int)(t & 1);
+    const bool stamp = p.tl && blockIdx.x == 0 && t < TL_TILES && tid == 0;
+    if (stamp) p.tl[t * 8 + 0] = clock64();
+    const uint32_t sa = smem_u32(sW), sb = smem_u32(sB + (size_t)buf * 2 * BH);
+    wgmma_fence();
+#pragma unroll 1
+    for (int q = 0; q < ksteps; ++q) {
+      const uint32_t ko = (uint32_t)(q >> 1) * SLOT_BYTES + (uint32_t)(q & 1) * 32;   // slot block, then 32 B inside the row
+      const uint64_t ahi = wgmma_desc_sw64(sa + a_off + ko), alo = wgmma_desc_sw64(sa + WH + a_off + ko);
+      const uint64_t bhi = wgmma_desc_sw64(sb + ko), blo = wgmma_desc_sw64(sb + BH + ko);
+      wgmma_f16_n128(d, alo, bhi, q ? 1u : 0u);                 // small terms first
+      wgmma_f16_n128(d, ahi, blo, 1u);
+      wgmma_f16_n128(d, ahi, bhi, 1u);
+    }
+    wgmma_commit();
+    if (t + 1 < T) {
+      build(t + 1, buf ^ 1);
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    }
+    if (stamp) p.tl[t * 8 + 1] = clock64();
+    wgmma_wait<0>();
+    wgmma_hold(d);
+    if (stamp) p.tl[t * 8 + 2] = clock64();
+
+    const long item = blockIdx.x + (t / nblocks) * gridDim.x;
+    const int nb = (int)(t % nblocks), n0 = nb * TN;
+    const bool edge = n0 + TN > p.N;
+#pragma unroll
+    for (int rh = 0; rh < 2; ++rh) {
+      const float* al = MU ? p.alpha + (size_t)rs[rh] * p.Npad_alpha : nullptr;
+      __half* shi = wst + (size_t)((lane >> 2) + 8 * rh) * OLDH;
+#pragma unroll
+      for (int blk = 0; blk < TN / 8; ++blk) {
+        const int col = blk * 8 + cq, n = n0 + col;
+        float2 r2 = fmul2(make_float2(d[blk * 4 + rh * 2], d[blk * 4 + rh * 2 + 1]), scl2[rh]);
+        r2.x = fmaxf(r2.x, 0.f);               // the (hi, lo) products can leave -1 ulp at coincident points
+        r2.y = fmaxf(r2.y, 0.f);
+        float2 kk = kernel_pair_fast_t<KIND>(r2);
+        if (edge) {                            // padded observations carry no covariance
+          if (n >= p.N) kk.x = 0.f;
+          if (n + 1 >= p.N) kk.y = 0.f;
+        }
+        if (MU) {
+          const float2 a = make_float2(n < p.N ? __ldg(al + n) : 0.f, n + 1 < p.N ? __ldg(al + n + 1) : 0.f);
+          v[rh] = ffma2(kk, a, v[rh]);
+        }
+        const float2 val = fmul2(kk, a2s[rh]);
+        const __half2 h2 = __floats2half2_rn(val.x, val.y);
+        const float2 hf = __half22float2(h2);
+        *reinterpret_cast<__half2*>(shi + col) = h2;
+        *reinterpret_cast<__half2*>(shi + 16 * OLDH + col) = __floats2half2_rn(val.x - hf.x, val.y - hf.y);
+      }
+    }
+    __syncwarp();
+    // coalesced write-out: row i of the warp's 16; lanes 0-15 store its hi, lanes 16-31 its lo, 16 bytes each
+#pragma unroll 4
+    for (int i = 0; i < 16; ++i) {
+      const int L = wg * 64 + (warp & 3) * 16 + i;
+      const int j = L / p.S, s = L - j * p.S;
+      const int crow = (int)item * p.J + j;               // candidate row inside the chunk
+      if (j < p.J && crow < p.mc_used) {
+        const int seg = lane >> 4, piece = lane & 15;
+        const uint4 dv = *reinterpret_cast<const uint4*>(wst + (size_t)(seg * 16 + i) * OLDH + piece * 8);
+        __half* dst = (seg ? p.klo : p.khi) + ((size_t)s * p.Mc + crow) * p.Np + n0 + piece * 8;
+        *reinterpret_cast<uint4*>(dst) = dv;
+      }
+    }
+    __syncwarp();
+    if (MU && nb == nblocks - 1) {                       // the item's last tile: mean partials of its rows
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        float m = v[rh].x + v[rh].y;
+        m += __shfl_xor_sync(0xffffffffu, m, 1);
+        m += __shfl_xor_sync(0xffffffffu, m, 2);
+        const int crow = (int)item * p.J + rj[rh];
+        if ((lane & 3) == 0 && rj[rh] < p.J && crow < p.mc_used) p.mu_partial[(size_t)rs[rh] * p.Mc + crow] = m;
+        v[rh] = make_float2(0.f, 0.f);
+      }
+    }
+    if (stamp) p.tl[t * 8 + 3] = clock64();
+    __syncthreads();   // buffer buf is free for tile t + 2, and tile t + 1's operand is complete
   }
 }
 
@@ -479,8 +315,8 @@ bool kxt_tc_supported(int D, int S) {
   return ktc::smem_bytes(ktc::slots(S, Dp) * Dp, S) <= (size_t)227 * 1024;
 }
 // Worth it?  An accumulator row is one (candidate slot, sample) pair and at most 3 slots fit the operand stage, so with few
-// samples most of the 128 TMEM lanes (= epilogue threads) idle: S = 5 uses 15 lanes and the SIMT generator is 3x faster there
-// (22 vs 6.6 ms per step of the 8-GPU per-rank shape); from half the lanes on the tensor-core generator wins.
+// samples most of the 128 accumulator rows are empty (S = 5 uses 15) while the epilogue still walks all of them; the
+// tensor-core generator is chosen from half the rows on (SMK_KXT_TC_MIN_LANES overrides the threshold).
 bool kxt_tc_preferred(int D, int S) {
   static int min_lanes = -1;
   if (min_lanes < 0) { const char* e = getenv("SMK_KXT_TC_MIN_LANES"); min_lanes = e ? atoi(e) : 64; }

@@ -30,7 +30,7 @@ __global__ void __launch_bounds__(256) potrf_diag_kernel(int Npad, int jb, T* __
 
 // ------------------------------------------------------------------------------------------ panel
 // L_Ij = A_Ij L_jj^-T by block substitution, 32 rows per CTA (diag.cuh: panel_sub_block); optional tf32 (hi, lo) copies
-// of the finished panel for the tcgen05 update.  grid = (rows below / 32, 1, S).
+// of the finished panel for the tensor-core update.  grid = (rows below / 32, 1, S).
 template <typename T>
 __global__ void __launch_bounds__(256) potrf_panel_kernel(int Npad, int jb, T* __restrict__ A,
                                                            const T* __restrict__ winv, T* __restrict__ hi = nullptr,
@@ -140,7 +140,7 @@ int potrf_lower_batched(int Npad, int S, T* A, T* winv, int* info, cudaStream_t 
 }
 
 // ---- left-looking variant with the rank-(jb*NB) update of each block-column pair on the tensor cores (float32):
-//   update(jb)  : A[rows >= jb][cols jb, jb+1] -= L[rows, 0:jb] L[jb:jb+2, 0:jb]^T     tcgen05 3xTF32 (predict_tc.cu)
+//   update(jb)  : A[rows >= jb][cols jb, jb+1] -= L[rows, 0:jb] L[jb:jb+2, 0:jb]^T     wgmma 3xTF32 (predict_tc.cu)
 //   diag, panel : as above; the panel kernel also writes the tf32 hi/lo copies the next updates read through TMA
 //   column jb+1 is brought up to date w.r.t. column jb by one rank-NB SIMT update.
 int tc_chol_update(int Npad, int S, int jb, int ncols, float* A, const float* lhi, const float* llo, cudaStream_t st);

@@ -1,8 +1,8 @@
 // potrf_ll.cu -- float64 batched Cholesky for the slice-sampler log-likelihood (f2; reference: the spla.cholesky inside
 // every logprob closure, OPT:637, 659, 690, ~50 D/8 calls per hyper-sample, thousands per next() at N = 4096).
 //
-// Round 1 ran this on the generic SIMT factorisation (NB = 64, 4 x 4 register tiles): 8.3 ms per N = 4096 matrix,
-// 2.8 TFLOP/s.  This file is the dedicated path:
+// The generic SIMT factorisation (NB = 64, 4 x 4 register tiles) is far from the fp64 tensor rate here, and a single
+// matrix is bound by its chain of diagonal steps.  This file is the dedicated path:
 //   * NB = 128 block columns in pairs, right-looking, look-ahead on three streams: while the rank-256 update of the
 //     trailing matrix (pair j) runs in the background, the next pair's diagonal blocks and panels are already being
 //     factored, and of the look-ahead updates only the one 128 x 128 block the next diagonal kernel reads stays on
@@ -177,7 +177,7 @@ __global__ void __launch_bounds__(256) dgemm_nt_kernel(GemmArgs g) {
 
 // The one update the NEXT diagonal kernel waits for: block (b, b) -= P P^T with P = rows of block b, columns [k0, k0 + K) of
 // the factor (K = 128 after one panel, 256 for the look-ahead of a pair).  On the 32-row GEMM above (4 CTAs, 256 - 512
-// dependent DMMAs per warp) this took 12 - 18 us of every spine step (ncu launch list r02).  Here: one CTA per 32 x 32 tile
+// dependent DMMAs per warp) this is a long serial chain on every spine step.  Here: one CTA per 32 x 32 tile
 // of the lower triangle (10 CTAs per matrix), both operand strips loaded in one burst of cp.async (every load in flight at
 // once), then K / 4 DMMAs per 8 x 8 tile in two independent chains -- 64 - 128 DMMAs per warp.
 constexpr int DBU_MAXK = 256;
@@ -237,9 +237,9 @@ static void launch_gemm(const GemmArgs& g, int tiles_m, int tiles_n, int S, cuda
 }
 
 // The background update: 128 x 128 tiles of the lower triangle (nt per side) of S matrices as a grid-stride loop over at
-// most `ctas` CTAs.  Two things make room for the spine next to it (ptxas: 166 registers -> one CTA per SM):
-//   * ctas < number of SMs: the diagonal kernel (186 registers x 256 threads) cannot share an SM with this kernel, and a
-//     tile of it runs ~45 us -- launched over all SMs it made every diagonal block wait for a tile to drain;
+// most `ctas` CTAs.  Two things make room for the spine next to it (its register use allows one CTA per SM):
+//   * ctas < number of SMs: the diagonal kernel cannot share an SM with this kernel (registers), and a tile of it runs
+//     long -- launched over all SMs it would make every diagonal block wait for a tile to drain;
 //   * a 2-stage ring (82 KB): the panel kernel (138 KB) and the 32-row GEMMs (77 KB) fit beside it on the same SM.
 template <int ST>
 static void launch_gemm_background_st(GemmArgs g, int nt, int S, int ctas, cudaStream_t st) {
@@ -316,7 +316,7 @@ static int enqueue(int Npad, int S, double* A, double* W, int* info, Streams& ss
   //   near (urgent): everything else of the two block columns while the diagonal kernels run: panel rest j, rest of column
   //                  j+1, panel rest j+1, then the look-ahead columns j+2 (panel head j+2 waits for it) and j+3;
   //   side (background): the rank-256 update of everything to the right of the next pair.
-  // A single matrix is bound by this spine, not by flops (22.9 Gflop at N = 4096 would take 0.6 ms at the DMMA peak).
+  // A single matrix is bound by this spine, not by flops (22.9 Gflop at N = 4096 is 0.34 ms at the H100 SXM data-sheet fp64 tensor rate of 67 TFLOP/s).
   auto gemm_args = [&](int jcol, int K, int row_blk, int col_blk, int tri) {
     GemmArgs g{};
     g.A = A + (long)jcol * NB; g.lda = Npad; g.a_stride = as;

@@ -1,20 +1,20 @@
-// predict_tc.cu -- tensor-core (tcgen05 / TMEM / TMA) version of the fused predict stage, and the tensor-core variants
+// predict_tc.cu -- tensor-core (wgmma / TMA) version of the fused predict stage, and the tensor-core variants
 // of the two N^3 factor steps that share its kernel.
 //
 // Same contract as predict.cu (reference spans OPT:536, 544, 547-548), different dataflow:
-//   1. trtri   : Linv = L^-1 explicitly (row-block recurrence on tcgen05, mode 3; SIMT version for small N) -- removes the
+//   1. trtri   : Linv = L^-1 explicitly (row-block recurrence on wgmma, mode 3; SIMT version for small N) -- removes the
 //                row-block dependency chain of the triangular solve: beta = Linv * Kx is one dense (lower-trapezoidal)
 //                contraction.  Kept as a tf32 (hi, lo) pair of float arrays (hi = tf32 round-to-nearest of x, lo = x - hi, exact).
 //   2. pack    : GEMM-operand copy of Linv: per-sample power-of-two scale 2^eb (largest |entry| -> [2^14, 2^15)) and the
 //                round-to-nearest fp16 (hi, lo) pair (linv_pack_f16).
 //   3. kxt     : Kxt[s][c][n] = amp2 k(X_n, C_c) * 2^ea for a chunk of candidates, candidate-major (n contiguous, i.e.
 //                K-major for the MMA) as an fp16 (hi, lo) pair; fused mu[c] = sum_n alpha[n] Kx[c][n] + mean.
-//                (kxt_kernel below: packed-float32 SIMT; kxt_tc.cu: opt-in tensor-core generator.)
+//                (kxt_kernel below: SIMT, the default; kxt_tc.cu: opt-in tensor-core generator.)
 //   4. mma     : per (sample, 128-candidate tile, row-group pair):  D[c][i] = sum_n Kxt[c][n] * Linv[i][n]
-//                as 3 x FP16 (lo*hi + hi*lo + hi*hi) with tcgen05.mma.kind::f16, fp32 accumulation, operands staged by
-//                TMA (64-byte swizzle, 4 stages), accumulators in TMEM (2 x 256 columns, double-buffered against the
-//                epilogue); epilogue = tcgen05.ld, un-scale by 2^-(ea+eb), per-lane sum of squares (one candidate per
-//                TMEM lane: no cross-thread reduction), partial sums per row-group pair.
+//                as 3 x FP16 (lo*hi + hi*lo + hi*hi) with wgmma m64n256k16, fp32 accumulation, operands staged by
+//                TMA (64-byte swizzle, 4 stages) by a producer warpgroup, two consumer warpgroups with the 128 x 256
+//                accumulator in registers; epilogue = un-scale by 2^-(ea+eb), sum of squares per candidate row (over
+//                the 4 lanes that share a row), partial sums per row-group pair.
 //   5. finish  : var = amp2 (1 + 1e-6) - sum_p partial[p]
 // Why a split at all: a single TF32/FP16 pass (11-bit significand) cannot resolve var = amp2 - |beta|^2 (it goes negative
 // on the reference's own test problems).  Why fp16 rather than tf32 halves: same significand, twice the tensor rate; the
@@ -310,8 +310,8 @@ __global__ void __launch_bounds__(256, 2) kxt_kernel(int kind, int N, int Np, in
           for (int rr = 0; rr < 4; ++rr)
 #pragma unroll
             for (int c = 0; c < 4; ++c) {
-              const float2 df = __fadd2_rn(a[rr], b[c]);
-              acc[g * 4 + rr][c] = __ffma2_rn(df, df, acc[g * 4 + rr][c]);
+              const float2 df = fadd2(a[rr], b[c]);
+              acc[g * 4 + rr][c] = ffma2(df, df, acc[g * 4 + rr][c]);
             }
         }
       }
@@ -338,8 +338,8 @@ __global__ void __launch_bounds__(256, 2) kxt_kernel(int kind, int N, int Np, in
             if (n >= N) kk.x = 0.f;
             if (n + 1 >= N) kk.y = 0.f;
           }
-          mdot[r] = __ffma2_rn(av[c], kk, mdot[r]);
-          const float2 v = __fmul2_rn(kk, a2s);
+          mdot[r] = ffma2(av[c], kk, mdot[r]);
+          const float2 v = fmul2(kk, a2s);
           hh[q] = __floats2half2_rn(v.x, v.y);
           const float2 hf = __half22float2(hh[q]);
           ll[q] = __floats2half2_rn(v.x - hf.x, v.y - hf.y);
@@ -366,56 +366,30 @@ __global__ void __launch_bounds__(256, 2) kxt_kernel(int kind, int N, int Np, in
   }
 }
 
-// ================================================================================================= tcgen05 kernel
+// ================================================================================================= wgmma kernel
 namespace tc {
-constexpr int BM = 128;        // candidates per tile (TMEM lanes, MMA M)
-constexpr int BN = 256;        // rows of Linv per group (MMA N, TMEM columns per accumulator)
+constexpr int BM = 128;        // candidates per tile (MMA M: two consumer warpgroups of 64 rows)
+constexpr int BN = 256;        // rows of Linv per group (MMA N: 64 x 256 fp32 accumulator per warpgroup, in registers)
 // Operand rows in shared memory are one 64-byte swizzle span: 16 tf32 (modes 2, 3: Cholesky update, triangular inverse)
 // or 32 fp16 (modes 0, 1: predict) -- identical tile bytes, descriptors and TMA box bytes for both element types; one
-// tcgen05.mma consumes 32 bytes of k (8 tf32 / 16 fp16), i.e. two MMAs per product per stage.
+// wgmma consumes 32 bytes of k (8 tf32 / 16 fp16), i.e. two MMAs per product per stage.
 constexpr int BK = 16;         // k per stage, tf32 elements
 constexpr int BK16 = 32;       // k per stage, fp16 elements
-constexpr int STAGES = 4;      // 4 x 48 KB: a TMA refill (~1.3 us from HBM) hides behind 3 stages of MMA
+constexpr int STAGES = 4;      // 4 x 48 KB: a TMA refill from HBM hides behind 3 stages of MMA
 constexpr int ROW_BYTES = BK * 4;                  // swizzle span = operand row in shared memory
 static_assert(ROW_BYTES == 64 && BK16 * 2 == ROW_BYTES, "operand rows must be one 64B swizzle span in both element types");
-constexpr int UK_BYTES = 32;                       // k bytes per tcgen05.mma (kind::tf32: 8 x 4 B, kind::f16: 16 x 2 B)
+constexpr int UK_BYTES = 32;                       // k bytes per wgmma (tf32: 8 x 4 B, f16: 16 x 2 B)
 constexpr int A_BYTES = BM * ROW_BYTES;   // 8 KB
 constexpr int B_BYTES = BN * ROW_BYTES;   // 16 KB
 constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;   // hi + lo of both operands: 48 KB
-constexpr int THREADS = 192;   // warp 0: TMA, warp 1: MMA + TMEM alloc, warps 2-5: epilogue
+constexpr int CONSUMERS = 2;   // warpgroups 1 and 2: MMA + epilogue, rows 64 wg .. 64 wg + 63 of the tile
+constexpr int THREADS = (CONSUMERS + 1) * 128;     // warpgroup 0: TMA (one thread issues, the rest give up registers)
+// Register split (setmaxnreg): 384 threads leave 168 registers per thread by default, which spills the consumers'
+// 128-float accumulator; the producer warpgroup drops to 40 and the consumers take 232 (128 x 40 + 256 x 232 <= 64 K).
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+static_assert(128 * PRODUCER_REGS + CONSUMERS * 128 * CONSUMER_REGS <= 65536, "register file");
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 
-// K-major swizzled operand tile: rows of ROW_BYTES, 8-row swizzle atoms (SBO = 8 rows), LBO unused (=1).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;                                  // leading byte offset (ignored for swizzled K-major)
-  d |= (uint64_t)((8 * ROW_BYTES) >> 4) << 32;             // stride byte offset: 8 rows
-  d |= (uint64_t)1 << 46;                                  // descriptor version (Blackwell)
-  d |= (uint64_t)4 << 61;                                  // SWIZZLE_64B
-  return d;
-}
-// kind::tf32, fp32 accumulate, A and B K-major, M = 128, N = 256
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(kIdesc), "r"(accumulate)
-      : "memory");
-}
-// kind::f16 with fp16 A and B (format 0), fp32 accumulate
-constexpr uint32_t kIdescF16 = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(kIdescF16), "r"(accumulate)
-      : "memory");
-}
 struct Args {
   int S, Np, Mc, ntiles, npairs, ngroups, ldp;   // Mc = candidates per chunk (multiple of 128); ldp = partial stride
   float* partial;                                 // [npairs][S][ldp]
@@ -484,51 +458,39 @@ __global__ void __launch_bounds__(THREADS, 1)
 predict_tc_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constant__ CUtensorMap mAlo,
                   const __grid_constant__ CUtensorMap mBhi, const __grid_constant__ CUtensorMap mBlo, Args p) {
   extern __shared__ unsigned char smem_raw[];
-  // 1024-byte alignment required by the 128B swizzle atoms
-  unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // 1 KB alignment of the operand tiles (swizzle atoms), by offset so the pointer keeps its shared address space
+  unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(base + STAGES * STAGE_BYTES);
   uint64_t* full = bars;                 // [STAGES]  TMA bytes landed: operands ready for the MMA
-  uint64_t* empty = bars + STAGES;       // [STAGES]  stage consumed (tcgen05.commit)
-  uint64_t* tfull = bars + 2 * STAGES;   // [2]
-  uint64_t* tempty = tfull + 2;          // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  uint64_t* empty = bars + STAGES;       // [STAGES]  stage consumed by every consumer warp
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CONSUMERS * 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
   const long nitems = (long)p.S * p.ntiles * (p.mode <= 1 ? p.npairs : 1);
+  const int bk = p.f16 ? BK16 : BK;
   // mode 0 item order (s, tile, pair): consecutive items share (s, tile) so the pair-blocks of one candidate tile run
   // concurrently on neighbouring SMs and hit L2 for the Kxt slab.
-  if (warp == 0) {
-    if (lane == 0) {
-      // A (cross-covariance slab of one candidate tile, 2 MB) is read by the 8 row-group-pair CTAs of that tile at
-      // different times: EVICT_FIRST made 7 of the 8 reads come from HBM (ncu r01: 103 GB read per launch vs 24 GB
-      // algorithmic); mode 0 therefore keeps it under the normal policy.  Modes 2/3 stream A once.
-      // (SMK_TC_A_EVICT_FIRST=1 restores the old hint for A/B measurements.)
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+    if (warp == 0 && lane == 0) {
+      // A (cross-covariance slab of one candidate tile) is read by the row-group-pair CTAs of that tile at different
+      // times, so mode 0 keeps it under the normal policy (EVICT_FIRST sends most of those reads to HBM).  Modes 2/3
+      // stream A once.  (SMK_TC_A_EVICT_FIRST=1 selects EVICT_FIRST for A/B measurements.)
       const uint64_t hintA = (p.mode == 0 && !p.a_evict_first) ? 0x1000000000000000ull : 0x12F0000000000000ull;   // EVICT_NORMAL : EVICT_FIRST
       const uint64_t hintB = 0x14F0000000000000ull;   // EVICT_LAST : the B operand is re-read by many items
       int stage = 0;
       uint32_t phase = 0;
-      const int bk = p.f16 ? BK16 : BK;
       for (long w = blockIdx.x; w < nitems; w += gridDim.x) {
         for (int h = 0; h < 2; ++h) {
           const Item it = get_item(p, w, h);
           if (!it.valid) break;
           for (int kc = 0; kc < it.nk; ++kc) {
-            mbar_wait_relaxed(&empty[stage], phase ^ 1, 64);   // the TMA thread sleeps until a stage is free (4 stages x ~0.4 us of MMAs ahead)
+            mbar_wait_relaxed(&empty[stage], phase ^ 1, 64);
             unsigned char* sb = base + stage * STAGE_BYTES;
             const int kk = it.k0 + kc * bk;
             mbar_expect_tx(&full[stage], STAGE_BYTES);
@@ -541,155 +503,150 @@ predict_tc_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0, buf = 0, bphase = 0;
-      for (long w = blockIdx.x; w < nitems; w += gridDim.x) {
-        for (int h = 0; h < 2; ++h) {
-          const Item it = get_item(p, w, h);
-          if (!it.valid) break;
-          mbar_wait(&tempty[buf], bphase ^ 1);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t d = tmem_base + buf * BN;
-          for (int kc = 0; kc < it.nk; ++kc) {
-            mbar_wait(&full[stage], phase);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t sa = smem_u32(base + stage * STAGE_BYTES);
-            const uint64_t ahi = umma_desc(sa), alo = umma_desc(sa + A_BYTES);
-            const uint64_t bhi = umma_desc(sa + 2 * A_BYTES), blo = umma_desc(sa + 2 * A_BYTES + B_BYTES);
-            if (p.f16) {
-#pragma unroll
-              for (int k = 0; k < ROW_BYTES / UK_BYTES; ++k) {
-                const uint64_t ko = (uint64_t)((k * UK_BYTES) >> 4);   // advance inside the swizzle atom (16 B units)
-                umma_f16(d, alo + ko, bhi + ko, (kc | k) ? 1u : 0u);   // small terms first
-                umma_f16(d, ahi + ko, blo + ko, 1u);
-                umma_f16(d, ahi + ko, bhi + ko, 1u);
-              }
-            } else {
-#pragma unroll
-              for (int k = 0; k < ROW_BYTES / UK_BYTES; ++k) {
-                const uint64_t ko = (uint64_t)((k * UK_BYTES) >> 4);
-                umma_tf32(d, alo + ko, bhi + ko, (kc | k) ? 1u : 0u);
-                umma_tf32(d, ahi + ko, blo + ko, 1u);
-                umma_tf32(d, ahi + ko, bhi + ko, 1u);
-              }
-            }
-            umma_commit(&empty[stage]);
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-          }
-          umma_commit(&tfull[buf]);
-          buf ^= 1;
-          if (buf == 0) bphase ^= 1;
-        }
-      }
-    }
-  } else {
-    // epilogue warps 2..5 own TMEM lane quarters (warp % 4); lane = row of the accumulator tile
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    uint32_t buf = 0, bphase = 0;
-    for (long w = blockIdx.x; w < nitems; w += gridDim.x) {
-      float acc = 0.f, accm = 0.f;
-      Item it0 = get_item(p, w, 0);
-      for (int h = 0; h < 2; ++h) {
-        const Item it = get_item(p, w, h);
-        if (!it.valid) break;
-        // undo the exact power-of-two operand scaling of the fp16 path
-        const float scl = p.f16 ? ldexpf(1.f, -(kx_exp(p.amp2[it.s]) + p.bexp[it.s])) : 1.f;
-        mbar_wait_relaxed(&tfull[buf], bphase, 1000);        // epilogue warps sleep through the item's MMAs (tens of us)
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t t0 = tmem_base + ((uint32_t)(q * 32) << 16) + buf * BN;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-          uint32_t r[32];
-          tmem_ld32(t0 + c0, r);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          if (p.mode == 0) {
-            if (p.z) {                          // predictive mean from the same accumulator: mu - mean = alpha . kx = z . beta
-              const float4* zq = reinterpret_cast<const float4*>(p.z + (long)it.s * p.Np + it.g * BN + c0);
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                const float4 z4 = __ldg(zq + (j >> 2));     // same address in every lane: broadcast
-                const float v0 = __uint_as_float(r[j]) * scl, v1 = __uint_as_float(r[j + 1]) * scl;
-                const float v2 = __uint_as_float(r[j + 2]) * scl, v3 = __uint_as_float(r[j + 3]) * scl;
-                acc = fmaf(v0, v0, acc); acc = fmaf(v1, v1, acc); acc = fmaf(v2, v2, acc); acc = fmaf(v3, v3, acc);
-                accm = fmaf(v0, z4.x, accm); accm = fmaf(v1, z4.y, accm); accm = fmaf(v2, z4.z, accm); accm = fmaf(v3, z4.w, accm);
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                float v = __uint_as_float(r[j]) * scl;
-                acc = fmaf(v, v, acc);
-              }
-            }
-            if (p.dbg) {
-              float* o = p.dbg + ((long)it.s * p.Mc + it.tile * BM + row) * p.Np + it.g * BN + c0;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) o[j] = __uint_as_float(r[j]) * scl;
-            }
-          } else if (p.mode == 1) {
-            const int gc = p.c_begin + it.tile * BM + row;
-            if (gc < p.M) {
-              const float mu0 = p.mean[it.s];
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const int f = it.g * BN + c0 + j;
-                if (f < p.F) p.mu_f[((long)it.s * p.F + f) * p.ldm + gc] = fmaf(__uint_as_float(r[j]), scl, mu0);
-              }
-            }
-          } else if (p.mode == 2) {
-            if (c0 < p.ncols) {
-              float* c = p.Cmat + ((long)it.s * p.Npad + (long)(p.jb + it.tile) * BM + row) * p.Npad + (long)p.jb * BM + c0;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                float4 v = *reinterpret_cast<float4*>(c + j);
-                v.x -= __uint_as_float(r[j]); v.y -= __uint_as_float(r[j + 1]);
-                v.z -= __uint_as_float(r[j + 2]); v.w -= __uint_as_float(r[j + 3]);
-                *reinterpret_cast<float4*>(c + j) = v;
-              }
-            }
-          } else {
-            const int jcol = it.tile * BN + c0;                 // first column of this chunk
-            if (jcol < p.K * BM) {
-              const long xr = ((long)it.s * p.Np + (long)p.K * BM + row) * p.Np + jcol;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                float v[4], hh[4], ll[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  v[e] = -__uint_as_float(r[j + e]);
-                  hh[e] = tf32_rn(v[e]);
-                  ll[e] = v[e] - hh[e];
-                }
-                *reinterpret_cast<float4*>(p.xhi + xr + j) = make_float4(hh[0], hh[1], hh[2], hh[3]);
-                *reinterpret_cast<float4*>(p.xlo + xr + j) = make_float4(ll[0], ll[1], ll[2], ll[3]);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {                   // transposed copy: lanes = consecutive k -> coalesced
-                  const long xt = ((long)it.s * p.Np + jcol + j + e) * p.Np + (long)p.K * BM + row;
-                  p.xthi[xt] = hh[e];
-                  p.xtlo[xt] = ll[e];
-                }
-              }
-            }
-          }
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty[buf]);
-        buf ^= 1;
-        if (buf == 0) bphase ^= 1;
-      }
-      if (p.mode == 0) {
-        p.partial[((long)it0.pr * p.S + it0.s) * p.ldp + it0.tile * BM + row] = acc;
-        if (p.z) p.mpartial[((long)it0.pr * p.S + it0.s) * p.ldp + it0.tile * BM + row] = accm;
-      }
-    }
+    return;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+
+  // ---- consumers: warpgroup 1 + wg owns accumulator rows 64 wg .. 64 wg + 63; this thread rows r0 and r0 + 8, and in
+  // every 8-column block the columns cq, cq + 1 (fragment layout: tc_common.cuh)
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
+  const int wg = (warp >> 2) - 1;
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const uint32_t a_off = (uint32_t)wg * 64 * ROW_BYTES;
+  float d[BN / 2];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (long w = blockIdx.x; w < nitems; w += gridDim.x) {
+    float acc[2] = {0.f, 0.f}, accm[2] = {0.f, 0.f};
+    const Item it0 = get_item(p, w, 0);
+    for (int h = 0; h < 2; ++h) {
+      const Item it = get_item(p, w, h);
+      if (!it.valid) break;
+      int prev = -1;
+      for (int kc = 0; kc < it.nk; ++kc) {
+        mbar_wait(&full[stage], phase);
+        const uint32_t sa = smem_u32(base + stage * STAGE_BYTES);
+        const uint64_t ahi = wgmma_desc_sw64(sa + a_off), alo = wgmma_desc_sw64(sa + A_BYTES + a_off);
+        const uint64_t bhi = wgmma_desc_sw64(sa + 2 * A_BYTES), blo = wgmma_desc_sw64(sa + 2 * A_BYTES + B_BYTES);
+        wgmma_fence();
+        if (p.f16) {
+#pragma unroll
+          for (int k = 0; k < ROW_BYTES / UK_BYTES; ++k) {
+            const uint64_t ko = (uint64_t)((k * UK_BYTES) >> 4);   // advance inside the swizzle atom (16 B units)
+            wgmma_f16_n256(d, alo + ko, bhi + ko, (kc | k) ? 1u : 0u);   // small terms first
+            wgmma_f16_n256(d, ahi + ko, blo + ko, 1u);
+            wgmma_f16_n256(d, ahi + ko, bhi + ko, 1u);
+          }
+        } else {
+#pragma unroll
+          for (int k = 0; k < ROW_BYTES / UK_BYTES; ++k) {
+            const uint64_t ko = (uint64_t)((k * UK_BYTES) >> 4);
+            wgmma_tf32_n256(d, alo + ko, bhi + ko, (kc | k) ? 1u : 0u);
+            wgmma_tf32_n256(d, ahi + ko, blo + ko, 1u);
+            wgmma_tf32_n256(d, ahi + ko, bhi + ko, 1u);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                   // the previous stage's MMAs are done: hand it back to TMA
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_hold(d);
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+      // undo the exact power-of-two operand scaling of the fp16 path
+      const float scl = p.f16 ? ldexpf(1.f, -(kx_exp(p.amp2[it.s]) + p.bexp[it.s])) : 1.f;
+      if (p.mode == 0) {
+        // predictive mean from the same accumulator when z is given: mu - mean = alpha . kx = z . beta
+        const float* zrow = p.z ? p.z + (long)it.s * p.Np + it.g * BN : nullptr;
+#pragma unroll
+        for (int nb = 0; nb < BN / 8; ++nb) {
+          const int c = nb * 8 + cq;
+          const float2 z2 = zrow ? __ldg(reinterpret_cast<const float2*>(zrow + c)) : make_float2(0.f, 0.f);
+#pragma unroll
+          for (int rh = 0; rh < 2; ++rh) {
+            const float v0 = d[nb * 4 + rh * 2] * scl, v1 = d[nb * 4 + rh * 2 + 1] * scl;
+            acc[rh] = fmaf(v0, v0, acc[rh]);
+            acc[rh] = fmaf(v1, v1, acc[rh]);
+            accm[rh] = fmaf(v0, z2.x, accm[rh]);
+            accm[rh] = fmaf(v1, z2.y, accm[rh]);
+            if (p.dbg) {
+              float* o = p.dbg + ((long)it.s * p.Mc + it.tile * BM + r0 + 8 * rh) * p.Np + it.g * BN + c;
+              o[0] = v0;
+              o[1] = v1;
+            }
+          }
+        }
+      } else if (p.mode == 1) {
+        const float mu0 = p.mean[it.s];
+#pragma unroll
+        for (int rh = 0; rh < 2; ++rh) {
+          const int gc = p.c_begin + it.tile * BM + r0 + 8 * rh;
+          if (gc >= p.M) continue;
+#pragma unroll
+          for (int nb = 0; nb < BN / 8; ++nb)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int f = it.g * BN + nb * 8 + cq + e;
+              if (f < p.F) p.mu_f[((long)it.s * p.F + f) * p.ldm + gc] = fmaf(d[nb * 4 + rh * 2 + e], scl, mu0);
+            }
+        }
+      } else if (p.mode == 2) {
+#pragma unroll
+        for (int nb = 0; nb < BN / 8; ++nb) {
+          const int c = nb * 8 + cq;
+          if (c >= p.ncols) continue;
+#pragma unroll
+          for (int rh = 0; rh < 2; ++rh) {
+            float2* cp = reinterpret_cast<float2*>(
+                p.Cmat + ((long)it.s * p.Npad + (long)(p.jb + it.tile) * BM + r0 + 8 * rh) * p.Npad + (long)p.jb * BM + c);
+            float2 v = *cp;
+            v.x -= d[nb * 4 + rh * 2];
+            v.y -= d[nb * 4 + rh * 2 + 1];
+            *cp = v;
+          }
+        }
+      } else {
+#pragma unroll
+        for (int nb = 0; nb < BN / 8; ++nb) {
+          const int jcol = it.tile * BN + nb * 8 + cq;      // first of this thread's two columns of X
+          if (jcol >= p.K * BM) continue;
+#pragma unroll
+          for (int rh = 0; rh < 2; ++rh) {
+            const int row = p.K * BM + r0 + 8 * rh;
+            const long xr = ((long)it.s * p.Np + row) * p.Np + jcol;
+            float hh[2], ll[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float v = -d[nb * 4 + rh * 2 + e];
+              hh[e] = tf32_rn(v);
+              ll[e] = v - hh[e];
+              const long xt = ((long)it.s * p.Np + jcol + e) * p.Np + row;   // transposed copy
+              p.xthi[xt] = hh[e];
+              p.xtlo[xt] = tf32_lo(v, hh[e]);
+            }
+            *reinterpret_cast<float2*>(p.xhi + xr) = make_float2(hh[0], hh[1]);
+            *reinterpret_cast<float2*>(p.xlo + xr) = make_float2(ll[0], ll[1]);
+          }
+        }
+      }
+    }
+    if (p.mode == 0) {             // row sums over the 4 lanes that share a row, fixed order
+#pragma unroll
+      for (int rh = 0; rh < 2; ++rh) {
+        float a = acc[rh], m = accm[rh];
+        a += __shfl_xor_sync(0xffffffffu, a, 1);
+        a += __shfl_xor_sync(0xffffffffu, a, 2);
+        m += __shfl_xor_sync(0xffffffffu, m, 1);
+        m += __shfl_xor_sync(0xffffffffu, m, 2);
+        if ((lane & 3) == 0) {
+          const long o = ((long)it0.pr * p.S + it0.s) * p.ldp + it0.tile * BM + r0 + 8 * rh;
+          p.partial[o] = a;
+          if (p.z) p.mpartial[o] = m;
+        }
+      }
+    }
   }
 }
 
@@ -872,7 +829,7 @@ __global__ void __launch_bounds__(256, 2) trtri_lt_kernel(int Npad, int K, const
       for (int e = 0; e < 4; ++e) {
         float x = acc[r][g * 4 + e];
         h.v[e] = tf32_hi(x);
-        l.v[e] = x - h.v[e];
+        l.v[e] = tf32_lo(x, h.v[e]);
       }
       const long o = off + (long)tile_row(ty, r) * Npad + g * 64 + tx * 4;
       st4(lthi + o, h);
@@ -891,7 +848,7 @@ __global__ void trtri_diag_store_kernel(int Npad, int Np, int K, const float* __
     float x = W[e], h = tf32_hi(x), l = x - h;
     long o = ((long)s * Np + (long)K * NB + i) * Np + (long)K * NB + k;
     long ot = ((long)s * Np + (long)K * NB + k) * Np + (long)K * NB + i;
-    xhi[o] = h; xlo[o] = l; xthi[ot] = h; xtlo[ot] = l;
+    xhi[o] = h; xlo[o] = l; xthi[ot] = h; xtlo[ot] = tf32_lo(x, h);
   }
 }
 
@@ -961,9 +918,8 @@ int trtri_split_tc(int Npad, int Np, int S, const float* L, const float* winv, f
 // Factor and invert in one call, pipelined: row block K of the inverse needs W_KK, row block K of L and the rows of the
 // inverse above it -- all final as soon as block column K of the factorisation is.  So the inversion runs ONE STEP BEHIND
 // the factorisation on a second stream instead of after it.  Both are chains of small dependent launches (32 block steps at
-// N = 4096); with few hyper-samples per GPU (the 8-GPU shape: 5) neither fills the machine and the two chains simply overlap
-// (3.5 + 3.8 ms one after the other).  With a full batch (40) each is throughput-bound and the overlap fills the bubbles
-// of the other's spine.
+// N = 4096); with few hyper-samples per GPU (the 8-GPU shape: 5) neither fills the machine and the two chains simply
+// overlap.  With a full batch (40) each is throughput-bound and the overlap fills the bubbles of the other's spine.
 int potrf_trtri_tc(int Npad, int Np, int S, float* A, float* winv, int* info, float* lhi, float* llo, float* linv_hi,
                    float* linv_lo, void* tws, size_t tws_bytes, cudaStream_t st) {
   if (Npad <= 0 || Npad % kNpadMult) return -1;
@@ -1025,8 +981,8 @@ int linv_alpha(int N, int Np, int S, const float* linv_hi, const float* linv_lo,
   return check_launch("linv_alpha");
 }
 
-// kxt(i+1) / MMA(i) overlap on two streams: measured SLOWER on B200 (both kernels share the 1 kW power cap: the clock
-// fell from 1515 to 1372 MHz and the step went from 474 to 543 ms), so it is opt-in (SMK_TC_OVERLAP=1).
+// kxt(i+1) / MMA(i) overlap on two streams: both kernels share the card's power budget, so running them together lowers
+// the clock for both and saves nothing on a power-capped card; opt-in (SMK_TC_OVERLAP=1), not measured on H100.
 static bool tc_overlap_enabled() {
   static int v = -1;
   if (v < 0) { const char* e = getenv("SMK_TC_OVERLAP"); v = (e && e[0] == '1') ? 1 : 0; }
@@ -1132,7 +1088,7 @@ int predict_tc_pregen(int kind, int N, int Np, int M, int D, int S, const float*
   int* fexp = reinterpret_cast<int*>(ahi + 2 * (size_t)S * Fp * Np);
   void* kws = reinterpret_cast<void*>(fexp + S);
   static int gen_env = -1;
-  if (gen_env < 0) { const char* e = getenv("SMK_KXT_IMPL"); gen_env = (e && !strcmp(e, "simt")) ? 0 : 1; }
+  if (gen_env < 0) { const char* e = getenv("SMK_KXT_IMPL"); gen_env = (e && !strcmp(e, "tc")) ? 1 : 0; }
   const bool gen_tc = gen_env == 1 && kxt_tc_preferred(D, S);
   PregenState& g = g_pregen;
   if (!g.stream) {
@@ -1186,11 +1142,11 @@ int predict_tc(int kind, int N, int Np, int M, int D, int S, const float* X, con
   __half* ahi = reinterpret_cast<__half*>(mpartial + (size_t)npairs * S * Mc);  // alpha^T hi | lo  [S][Fp][Np]
   __half* alo = ahi + (size_t)S * Fp * Np;
   int* fexp = reinterpret_cast<int*>(alo + (size_t)S * Fp * Np);
-  // generator: the tensor-core kernel of kxt_tc.cu (contraction over dimensions on tcgen05) wherever it applies (D <= 32,
-  // shared-memory budget permitting; 59 vs 73 ms per headline step on the same box, round 2) -- the packed-float32 SIMT
-  // kernel otherwise, or when asked for with SMK_KXT_IMPL=simt
+  // generator: the SIMT kernel above; SMK_KXT_IMPL=tc selects the tensor-core kernel of kxt_tc.cu (contraction over
+  // dimensions on wgmma) where it applies.  On an H100 SXM the SIMT kernel is the faster of the two at the headline
+  // (80 against 95 ms per step, S = 40), and the tensor-core one only loses ground with fewer samples.
   static int gen_env = -1;
-  if (gen_env < 0) { const char* e = getenv("SMK_KXT_IMPL"); gen_env = (e && !strcmp(e, "simt")) ? 0 : 1; }
+  if (gen_env < 0) { const char* e = getenv("SMK_KXT_IMPL"); gen_env = (e && !strcmp(e, "tc")) ? 1 : 0; }
   const bool gen_tc = gen_env == 1 && kxt_tc_preferred(D, S) && nbuf == 1;
   const int nmp = (gen_tc && !z) ? kxt_tc_ngroups(Np) : 0;
   void* kws = reinterpret_cast<void*>(fexp + S);

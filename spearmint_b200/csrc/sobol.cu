@@ -10,6 +10,8 @@
 
 namespace smk {
 
+int num_sms();
+
 template <typename T>
 __global__ void __launch_bounds__(256) sobol_kernel(int D, long n, long skip, const uint32_t* __restrict__ V,
                                                      T* __restrict__ out) {
@@ -41,7 +43,8 @@ int sobol_generate(int D, long n, long skip, const uint32_t* V, T* out, cudaStre
   if (skip + n - 1 >= (1L << 30)) return -3;           // the reference's MAXCOL = 30 limit ("Too many calls!")
   if (!V || !out) return -4;
   const long total = n * D;
-  const int blocks = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const long cap = 16L * num_sms();
+  const int blocks = (int)((total + 255) / 256 < cap ? (total + 255) / 256 : cap);
   const size_t smem = sizeof(uint32_t) * D * 30;
   static bool attr = false;
   if (!attr) {

@@ -1,5 +1,5 @@
-// tc_common.cuh -- device helpers shared by the tcgen05 kernels (predict_tc.cu, kxt_tc.cu): fp16 operand scaling /
-// splitting, fast stationary kernels on packed float32, and thin wrappers over the mbarrier / TMA / tcgen05 PTX.
+// tc_common.cuh -- device helpers shared by the tensor-core kernels (predict_tc.cu, kxt_tc.cu): fp16 operand scaling /
+// splitting, fast stationary kernels on float2 pairs, and thin wrappers over the mbarrier / TMA / wgmma PTX (sm_90a).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda.h>
@@ -14,7 +14,7 @@ namespace smk {
 // by an exact power of two that puts its largest |entry| in [2^14, 2^15) before the round-to-nearest split
 //     hi = fp16(x * 2^e),   lo = fp16(x * 2^e - hi)
 // (representation error <= 2^-23 |x| for entries within 2^-18 of the maximum, <= 2^-40 max|x| absolute below that;
-// tools/fp16_split_experiment.py, profiles/r01_fp16_split_experiment.md).  The epilogue multiplies the accumulator by
+// tools/fp16_split_experiment.py).  The epilogue multiplies the accumulator by
 // 2^-(ea + eb); the scaling is exact, so it changes nothing but the representable range.
 __host__ __device__ __forceinline__ int scale_exp(float amax) {
   int e;
@@ -36,8 +36,8 @@ __device__ __forceinline__ uint2 pack4(const __half (&v)[4]) {
 
 // Fast stationary kernels for the generator (float32): sqrt.approx / ex2.approx (MUFU, ~1-2 ulp) instead of the accurate
 // sqrtf/expf sequences -- their relative error (~2e-7) is at the level of the float32 rounding already carried by r2.
-// The kernel is issue-bound (ncu r01: 110 instructions per element, 73% issue-slot utilisation, FMA pipe 53%), so the
-// arithmetic is written with Blackwell's packed float32 instructions (FADD2 / FFMA2 / FMUL2: two lanes per issue slot).
+// Pairs of columns travel together as float2; Hopper has no packed float32 arithmetic, so the pair operations below are
+// two scalar instructions with the same rounding.
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -49,34 +49,39 @@ __device__ __forceinline__ float sqrt_approx(float x) {
   return y;
 }
 __device__ __forceinline__ float2 dup2(float x) { return make_float2(x, x); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
 template <int KIND>
 __device__ __forceinline__ float2 kernel_pair_fast_t(float2 r2) {      // same arithmetic, kind resolved at compile time
   constexpr float kL2E = 1.4426950408889634f;
   if (KIND <= 1) {
-    const float2 t = __fmul2_rn(r2, dup2(-0.5f * kL2E));
+    const float2 t = fmul2(r2, dup2(-0.5f * kL2E));
     return make_float2(ex2_approx(t.x), ex2_approx(t.y));
   }
   const float2 r = make_float2(sqrt_approx(r2.x), sqrt_approx(r2.y));
   constexpr float c = (KIND == 2) ? 1.7320508075688772f : 2.23606797749979f;
-  const float2 t = __fmul2_rn(r, dup2(-c * kL2E));
+  const float2 t = fmul2(r, dup2(-c * kL2E));
   const float2 e = make_float2(ex2_approx(t.x), ex2_approx(t.y));
-  float2 p = __ffma2_rn(r, dup2(c), dup2(1.f));
-  if (KIND == 3) p = __ffma2_rn(r2, dup2(5.0f / 3.0f), p);
-  return __fmul2_rn(p, e);
+  float2 p = ffma2(r, dup2(c), dup2(1.f));
+  if (KIND == 3) p = ffma2(r2, dup2(5.0f / 3.0f), p);
+  return fmul2(p, e);
 }
 __device__ __forceinline__ float2 kernel_pair_fast(int kind, float2 r2) {
   constexpr float kL2E = 1.4426950408889634f;
   if (kind <= 1) {                                            // SE / ARDSE: exp(-r2 / 2)
-    const float2 t = __fmul2_rn(r2, dup2(-0.5f * kL2E));
+    const float2 t = fmul2(r2, dup2(-0.5f * kL2E));
     return make_float2(ex2_approx(t.x), ex2_approx(t.y));
   }
   const float2 r = make_float2(sqrt_approx(r2.x), sqrt_approx(r2.y));
   const float c = (kind == 2) ? 1.7320508075688772f : 2.23606797749979f;
-  const float2 t = __fmul2_rn(r, dup2(-c * kL2E));
+  const float2 t = fmul2(r, dup2(-c * kL2E));
   const float2 e = make_float2(ex2_approx(t.x), ex2_approx(t.y));
-  float2 p = __ffma2_rn(r, dup2(c), dup2(1.f));               // Matern32: (1 + sqrt3 r) e^-sqrt3 r
-  if (kind == 3) p = __ffma2_rn(r2, dup2(5.0f / 3.0f), p);    // Matern52: (1 + sqrt5 r + 5/3 r2) e^-sqrt5 r
-  return __fmul2_rn(p, e);
+  float2 p = ffma2(r, dup2(c), dup2(1.f));               // Matern32: (1 + sqrt3 r) e^-sqrt3 r
+  if (kind == 3) p = ffma2(r2, dup2(5.0f / 3.0f), p);    // Matern52: (1 + sqrt5 r + 5/3 r2) e^-sqrt5 r
+  return fmul2(p, e);
 }
 
 namespace tc {
@@ -99,10 +104,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 // Same wait for threads that expect to wait LONG (a producer on a free stage, an epilogue warp on its next accumulator):
 // poll, then SLEEP for `ns` before the next poll, so the waiting warp stays out of the issue slots (and the power budget) of
-// the warps that are doing the work.  ncu of the generator (r02): with a bare try_wait loop SYNCS + YIELD + BRA were ~20 % of
-// all executed instructions; with try_wait's suspend-time hint the compiler's loop (SYNCS, NANOSLEEP, BRA) still ran 4.8e8
-// iterations per launch = 29 % of the executed instructions -- the hint does not keep the thread asleep.  An explicit sleep
-// of a few hundred nanoseconds costs at most that much latency per tile and removes the polling.
+// the warps that are doing the work.  A bare try_wait loop keeps issuing SYNCS / BRA instructions for as long as it
+// waits, and try_wait's suspend-time hint does not keep the thread asleep.  An explicit sleep of a few hundred
+// nanoseconds costs at most that much latency per tile and removes the polling.
 __device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity, uint32_t ns = 256) {
   uint32_t done;
   for (;;) {
@@ -131,20 +135,77 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// ------------------------------------------------------------------------------------------------------------ wgmma
+// Shared-memory matrix descriptor of a K-major operand tile in the 64-byte swizzle (rows of 64 bytes, 8-row atoms of
+// 512 bytes: stride byte offset 512; the leading byte offset is unused for swizzled K-major tiles).  The tile base must
+// be 512-byte aligned; a k step inside the 64-byte row is an advance of the start address (bytes >> 4).
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t saddr) {
+  uint64_t d = (uint64_t)((saddr >> 4) & 0x3FFF);
+  d |= (uint64_t)1 << 16;                                  // leading byte offset (unused)
+  d |= (uint64_t)(512 >> 4) << 32;                         // stride byte offset: 8 rows x 64 B
+  d |= (uint64_t)2 << 62;                                  // SWIZZLE_64B
+  return d;
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// The accumulator registers must not be reordered across the asynchronous MMAs that own them.
+template <int R>
+__device__ __forceinline__ void wgmma_hold(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D (+)= A * B^T for one warpgroup, fp32 accumulate, both operands K-major in shared memory (descriptors above);
+// scale_d == 0 starts a new accumulation.  Accumulator fragment of thread (warp w of the group, lane l), element i:
+// row 16 w + l / 4 + 8 ((i / 2) % 2), column 8 (i / 4) + 2 (l % 4) + i % 2.
+__device__ __forceinline__ void wgmma_f16_n256(float (&d)[128], uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a), "l"(b), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_tf32_n256(float (&d)[128], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a), "l"(b), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(scale_d));
 }
 
 }  // namespace tc

@@ -231,7 +231,7 @@ class GPEIEngine(object):
 
     def __init__(self, device=None, dtype=torch.float32):
         if not torch.cuda.is_available():
-            raise _lib.SmkError("spearmint_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise _lib.SmkError("spearmint_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         _lib.lib()
         self.device = torch.device(device if device is not None else "cuda:%d" % torch.cuda.current_device())
         torch.cuda.set_device(self.device)
@@ -240,11 +240,11 @@ class GPEIEngine(object):
         self.NB = _lib.lib().smk_block(self.esize)
         self._ws = None
         self._ws_tc = None
-        # fused-predict implementation: "tc" = tcgen05/TMEM/TMA 3xFP16 kernel (float32 in/out), "simt" = register-tiled FMA
+        # fused-predict implementation: "tc" = wgmma/TMA 3xFP16 kernel (float32 in/out), "simt" = register-tiled FMA
         self.predict_impl = os.environ.get("SMK_PREDICT_IMPL", "tc" if dtype == torch.float32 else "simt")
         if dtype != torch.float32:
             self.predict_impl = "simt"
-        # N^3 steps (Cholesky trailing update, triangular inverse): "tc" = tcgen05 3xTF32 left-looking variants
+        # N^3 steps (Cholesky trailing update, triangular inverse): "tc" = wgmma 3xTF32 left-looking variants
         self.factor_impl = os.environ.get("SMK_FACTOR_IMPL", "tc" if self.predict_impl == "tc" else "simt")
         # The explicit-inverse tensor-core chain is the path for LARGE factors.  Below tc_min_n observations the float32
         # blocked-substitution chain (SIMT Cholesky + SIMT predict) is used: it is 3-8x more accurate on the smooth,
@@ -253,8 +253,8 @@ class GPEIEngine(object):
         self.tc_min_n = int(os.environ.get("SMK_TC_MIN_N", "2048"))
         # opt-in accuracy guard of the tensor-core chain (csrc/guard.cu, _guarded_impl): a hyper-sample whose ESTIMATED EI
         # error exceeds this fraction of its EI scale is re-evaluated in float64.  The estimate is conservative (it
-        # over-predicts the measured error by up to 8x), so it is off by default (0) and meant for users whose problems are
-        # both large and badly conditioned.
+        # over-predicts the actual error), so it is off by default (0) and meant for users whose problems are both large
+        # and badly conditioned.
         self.guard_threshold = float(os.environ.get("SMK_TC_GUARD", "0"))
         self.last = {}
         self._deferred_info = []
@@ -264,8 +264,8 @@ class GPEIEngine(object):
         self._pool = {}      # (stream, shape, dtype) -> free tensors: the big per-call buffers are recycled, never re-allocated
         self._home = {}      # data_ptr -> stream the buffer belongs to
         self._side = None    # second stream: the factor chain of one half of the samples runs under the other half's GEMM
-        # measured: no gain (268.8 -> 272.6 ms at S=40, 37.8 -> 39.9 ms at S=5): the persistent GEMM and the generator leave no
-        # SM for the side stream's kernels to run on, and two groups double the launches.  Off unless asked for.
+        # the persistent GEMM and the generator leave no SM for the side stream's kernels to run on, and two groups double the
+        # launches.  Off unless asked for.
         self.overlap = os.environ.get("SMK_FACTOR_OVERLAP", "0") == "1"
         # tensor-core chain: factorisation and explicit inverse as one pipelined call (csrc/predict_tc.cu: potrf_trtri_tc);
         # SMK_FUSED_INVERSE=0 runs them one after the other (the two separate entry points)
@@ -273,9 +273,8 @@ class GPEIEngine(object):
         # Opt-in (SMK_MEAN_FROM_GEMM=1, SMK_PREGEN=1): predictive mean reduced in the GEMM epilogue (mu - mean = z . beta,
         # z = Linv (y - mean)) instead of in the generator (alpha . kx) -- the generator then depends on nothing the
         # factorisation produces, and the first candidate chunk is generated on a second stream WHILE K is factored and
-        # inverted.  Measured (profiles/r02_pregen_experiment.md): 2 % at 40 hyper-samples, nothing at 5 (the generator
-        # starves the factorisation's small kernels), and the mean inherits the tensor-core accumulation error of beta
-        # (headline 6.9e-4 -> 1.3e-3 of max EI, C5 1.3e-3 -> 3.3e-3): accuracy first, so both stay off.
+        # inverted.  The generator then competes with the factorisation's small kernels, and the mean inherits the
+        # tensor-core accumulation error of beta: accuracy first, so both stay off.
         self.mean_from_gemm = os.environ.get("SMK_MEAN_FROM_GEMM", "0") == "1"
         self.pregen_enabled = self.mean_from_gemm and os.environ.get("SMK_PREGEN", "0") == "1"
         self._helper64 = None
@@ -577,8 +576,7 @@ class GPEIEngine(object):
         of such a candidate (s^2 ~ noise + jitter, u ~ 0) then moves by about  0.5 phi(0) g sqrt(noise + 1e-6 amp2), which
         is kept per sample as the absolute bound p.gbound[s].  After every sweep the bound is compared with the largest EI
         of the sample (ei_prepared): a sample whose bound exceeds guard_threshold * max EI is re-evaluated on the float64
-        engine.  Well-conditioned problems (the headline: bound / max EI ~ 6e-4) never trip it; smooth low-dimensional ones
-        (C2, C4: ~5e-3) do.  Measured against actual errors in profiles/r02_precision_guard.md."""
+        engine.  Well-conditioned problems (the headline) do not trip it; smooth low-dimensional ones (C2, C4) do."""
         p.gbound, p.flagged, p.prep64 = None, None, None
         if self.guard_threshold > 0:
             # probes: the observed points with the lowest values -- the incumbent (the chooser's jitter cloud sits on it) and

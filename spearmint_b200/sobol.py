@@ -34,7 +34,7 @@ def sobol_device(dims, size, skip, device=None, dtype=None):
     """(size, dims) torch tensor on the device (row-major, what the engine's candidate buffer wants)."""
     import torch
     if not torch.cuda.is_available():
-        raise _lib.SmkError("spearmint_b200.sobol needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise _lib.SmkError("spearmint_b200.sobol needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     device = torch.device(device if device is not None else "cuda:%d" % torch.cuda.current_device())
     dtype = dtype or torch.float64
     if not 1 <= dims <= 1111:

@@ -231,7 +231,7 @@ def test_topk_matches_numpy(engines, M, k):
 # ------------------------------------------------------------------------------------------------ tensor-core predict
 @pytest.mark.parametrize("D,N,M", [(6, 100, 128), (8, 300, 1000), (3, 520, 257), (40, 260, 200)])
 def test_predict_tc_beta_and_moments(engines, D, N, M):
-    """tcgen05 3xFP16 path: the fp16 operand pack of L^-1 (scale + hi/lo), the dumped beta^T = Kx^T L^-T tile product
+    """wgmma 3xFP16 path: the fp16 operand pack of L^-1 (scale + hi/lo), the dumped beta^T = Kx^T L^-T tile product
     (descriptor / swizzle / pipeline / un-scaling check) and the resulting moments, against the oracle."""
     import torch
     from spearmint_b200 import _lib

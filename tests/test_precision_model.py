@@ -2,7 +2,7 @@
 the hardware's round-to-nearest, subnormal and range behaviour; products exact, as on the tensor cores):
 
 * the predict GEMM's scaled 3 x FP16 split is at least as accurate as the truncating 3 x TF32 split it replaced
-  (DESIGN.md section 6, profiles/r01_fp16_split_experiment.md), also when amp2 is far from 1;
+  (DESIGN.md section 6, tools/fp16_split_experiment.py), also when amp2 is far from 1;
 * the exact power-of-two scaling keeps every operand inside the fp16 range;
 * the sample-factored distance  r2_s = sum_d w_sd (x_d - c_d)^2  evaluated as split products is as accurate as the
   float32 FMA chain (tools/kxt_tc_precision_experiment.py)."""

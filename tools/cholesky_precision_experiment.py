@@ -1,5 +1,6 @@
-import numpy as np, scipy.linalg as spla, sys
-sys.path.insert(0,'/root/repo')
+import os, sys
+import numpy as np, scipy.linalg as spla
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import gp_oracle as O
 f32=lambda a: np.asarray(a,dtype=np.float32)
 def trunc_tf32(x):

@@ -3,8 +3,9 @@ instead of 3 x TF32?  fp16 has tf32's 11-bit significand but only 5 exponent bit
 an exact power of two that puts its largest |entry| in [2^14, 2^15); numpy float16 reproduces the round-to-nearest,
 subnormal and overflow behaviour of the hardware conversion.  Products are exact and accumulated in float64 here (the
 tensor core accumulates in fp32; that part is common to every variant and is covered by the fp32in row)."""
-import numpy as np, scipy.linalg as spla, sys
-sys.path.insert(0, '/root/repo')
+import os, sys
+import numpy as np, scipy.linalg as spla
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import gp_oracle as O
 
 def pow2_scale(x):

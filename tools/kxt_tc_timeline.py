@@ -7,7 +7,7 @@ from spearmint_b200 import _lib
 from spearmint_b200.engine import GPEIEngine, ptr, check, KINDS
 eng = GPEIEngine(device="cuda:0", dtype=torch.float32)
 L = _lib.lib()
-D, N, M, S = 32, 4096, 148 * 3 * 4, 40
+D, N, M, S = 32, 4096, 132 * 3 * 4, 40
 rs = np.random.RandomState(0)
 X, C = rs.rand(N, D), rs.rand(M, D)
 hs = [(0.0, 1e-3, 1.0, rs.uniform(0.3, 2.0, D)) for _ in range(S)]
@@ -27,11 +27,10 @@ for it in range(2):
     print("launch %d: %.3f ms for %d items x 32 tiles" % (it, ev0.elapsed_time(ev1), (Mc + 2) // 3))
 out = (ctypes.c_longlong * 512)()
 assert L.smk_debug_kxt_tc_timeline(out, 512) == 0
-tl = np.array(out[:], dtype=np.int64).reshape(64, 8)
+tl = np.array(out[:], dtype=np.int64).reshape(64, 8)[:, :4]
 t0 = tl[0, 0]
-print("tile  prod_start prod_end | iss_arrive iss_ready iss_commit | epi_wait epi_ready epi_done   (cycles from first stamp)")
+print("tile  mma_issue  next_q_built  mma_done  epilogue_done   (cycles from first stamp)")
 for t in range(40):
     print("%3d  " % t + " ".join("%9d" % (v - t0) for v in tl[t]))
-d = np.diff(tl[8:40, 4])
-print("issue period (commit to commit) median", np.median(d), " epi_ready - iss_commit median", np.median(tl[8:40, 6] - tl[8:40, 4]),
-      " epi busy (done - ready) median", np.median(tl[8:40, 7] - tl[8:40, 6]), " prod time median", np.median(tl[8:40, 1] - tl[8:40, 0]))
+print("tile period median", np.median(np.diff(tl[8:40, 0])), " q build median", np.median(tl[8:40, 1] - tl[8:40, 0]),
+      " MMA wait after the build median", np.median(tl[8:40, 2] - tl[8:40, 1]), " epilogue median", np.median(tl[8:40, 3] - tl[8:40, 2]))

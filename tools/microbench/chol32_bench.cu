@@ -1,6 +1,6 @@
 // chol32_bench.cu -- variants of the 32 x 32 warp Cholesky (the serial core of csrc/diag.cuh), one warp, clock64 per run,
 // cold (first execution of the code) and warm (second execution in the same launch).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o chol32_bench chol32_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o chol32_bench chol32_bench.cu
 #include <cmath>
 #include <cstdio>
 #include <vector>

@@ -1,6 +1,6 @@
 // diag_bench.cu -- phase timeline (clock64) and a standalone correctness check of the spine kernels of csrc/diag.cuh:
 // diag_factor_block (L, diagonal inverses), winv_assemble_block (W L = I), panel_sub_block (X L^T = A).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -DSMK_DIAG_TIMELINE -I../../spearmint_b200/csrc -o diag_bench diag_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -DSMK_DIAG_TIMELINE -I../../spearmint_b200/csrc -o diag_bench diag_bench.cu
 #include <cmath>
 #include <cstdio>
 #include <vector>

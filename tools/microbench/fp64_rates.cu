@@ -1,6 +1,6 @@
 // fp64_rates.cu -- measured fp64 issue rates on the device: DFMA (SIMT) vs DMMA (mma.sync.m8n8k4.f64).
 // Decides how the float64 Cholesky trailing update (slice-sampler log-likelihood, f2) is written.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_rates fp64_rates.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_rates fp64_rates.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,5 +1,6 @@
-import numpy as np, scipy.linalg as spla, sys
-sys.path.insert(0,'/root/repo')
+import os, sys
+import numpy as np, scipy.linalg as spla
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import gp_oracle as O
 def rnd_bits(x, bits):  # round to `bits` mantissa bits (incl. implicit) -- emulate tf32(11)/bf16(8)
     m, e = np.frexp(x); s = 2.0**bits
