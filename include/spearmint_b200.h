@@ -226,6 +226,32 @@ int smk_ei_sweep_f64(int M, int S, int F, const double* mu, const double* var, i
  * with the error bound of the explicit-inverse path).  smk_ei_colsum: ei_sum[j] += sum_s ei[s][j].                    */
 int smk_ei_colsum(int M, int S, const double* ei, int ldm, double* ei_sum, void* stream);
 
+/* ---- (5b) constrained EI (CONS = chooser/GPConstrainedEIChooser.py)
+ * smk_constraint_prob: p[s][j] = Phi(gain[s] * m[s][j]),  m[s][j] = amp2[s] k_s(X, C_j)' t_alpha[s]   (CONS:819-842)
+ *   X [N][D] every complete input (violations included), C [M][D], inv_ls/amp2 of the constraint GP (element type T);
+ *   t_alpha [S][Npad] = K_c^-1 ff, gain [S], p [S][ldm] and the optional m_out [S][ldm] are DOUBLE for both variants,
+ *   and so is the arithmetic (K_c^-1 ff has large entries of both signs: float32 kernel values lose m); Phi is
+ *   evaluated with an erfc tail.  The variants differ only in the element type of X, C, inv_ls and amp2.
+ * smk_ei_sweep_weighted: the contract of smk_ei_sweep without log_time, each per-sample EI (mean over the F fantasies)
+ *   multiplied by w[s][j] (double [S][ldm]: the p of smk_constraint_prob)  (CONS:878, 940).                          */
+/* smk_loglik_set_rhs_batched: smk_loglik_set_rhs with one right-hand side per batch item, y [S][ldy], and no mean
+ *   subtracted: the joint [amp2, ff] slice move of the classification GP moves ff with every proposal (CONS:1169-1190).
+ * smk_lower_matvec_f64: out = L z for the lower factor L [Npad][Npad] of smk_potrf_lower_batched_f64 (one matrix): the
+ *   direction of an elliptical-slice step (CONS:1241).                                                             */
+int smk_loglik_set_rhs_batched_f32(int N, int Npad, int S, const float* y, int ldy, float* A, void* stream);
+int smk_loglik_set_rhs_batched_f64(int N, int Npad, int S, const double* y, int ldy, double* A, void* stream);
+int smk_lower_matvec_f64(int N, int Npad, const double* L, const double* z, double* out, void* stream);
+int smk_constraint_prob_f32(int kind, int N, int Npad, int M, int D, int S, const float* X, const float* C,
+                            const float* inv_ls, const float* amp2, const double* t_alpha, const double* gain,
+                            double* p_out, double* m_out, int ldm, void* stream);
+int smk_constraint_prob_f64(int kind, int N, int Npad, int M, int D, int S, const double* X, const double* C,
+                            const double* inv_ls, const double* amp2, const double* t_alpha, const double* gain,
+                            double* p_out, double* m_out, int ldm, void* stream);
+int smk_ei_sweep_weighted_f32(int M, int S, int F, const float* mu, const float* var, int ldm, const float* best,
+                              const double* w, double* ei, double* ei_sum, unsigned long long* ei_max, void* stream);
+int smk_ei_sweep_weighted_f64(int M, int S, int F, const double* mu, const double* var, int ldm, const double* best,
+                              const double* w, double* ei, double* ei_sum, unsigned long long* ei_max, void* stream);
+
 /* ---- (6) selection: argsort(mean)[-k:] and argmax(mean)   (OPT:270-271, OPT:294)
  * score: [M].  idx_out[k]: indices of the k largest scores in ASCENDING score order (so
  * idx_out[k-1] is the argmax; ties resolved towards the lower index, numpy's first-max rule).

@@ -71,6 +71,7 @@ SIGNATURES = {
     "smk_linv_pack_f16": ([_i, _i, _p, _p, _p, _p, _p, _p], _i),
     "smk_predict_tc_f32": ([_i] * 6 + [_p] * 9 + [_i, _p, _p, _i, _p, _sz, _p, _i, _p, _p, _p, _i, _p], _i),
     "smk_predict_tc_pregen_f32": ([_i] * 6 + [_p] * 5 + [_sz, _i, _p], _i),
+    "smk_lower_matvec_f64": ([_i, _i, _p, _p, _p, _p], _i),
 }
 for _t in ("f32", "f64"):
     SIGNATURES.update({
@@ -87,6 +88,9 @@ for _t in ("f32", "f64"):
         "smk_ei_sweep_" + _t: ([_i, _i, _i, _p, _p, _i, _p, _p, _p, _p, _p, _p], _i),
         "smk_topk_" + _t: ([_i, _i, _p, _p, _p, _p, _sz, _p], _i),
         "smk_ei_grad_terms_" + _t: ([_i] * 7 + [_p] * 8, _i),
+        "smk_loglik_set_rhs_batched_" + _t: ([_i, _i, _i, _p, _i, _p, _p], _i),
+        "smk_constraint_prob_" + _t: ([_i] * 6 + [_p] * 8 + [_i, _p], _i),
+        "smk_ei_sweep_weighted_" + _t: ([_i, _i, _i, _p, _p, _i, _p, _p, _p, _p, _p, _p], _i),
     })
 
 

@@ -6,6 +6,8 @@
     ei_matrix(state, cand)                        -> (M, S) float64 numpy                        (OPT:331-341)
     top_mean_ei(state, cand, k)                   -> indices of the k largest mean-EI candidates, ascending (OPT:270, 294)
     refine_context(...)                           -> object with value_grad(x)                   (f1, OPT:360-525)
+    constrained_ei_matrix(kind, hs, constraint_hs, ff, comp, labels, pend, cand, vals, normals)
+                                                  -> (M, S) float64 numpy, constrained EI        (CONS:450-468)
 
 The chooser classes only talk to this interface, so the host logic (RNG order, state files, return protocol)
 can be unit-tested on a CPU-only box with a stand-in backend supplied by the test; the product always constructs
@@ -142,6 +144,64 @@ class DeviceBackend(object):
         if np.any(out < 0):                          # every score NaN: the reference's argmax would return index 0 of NaNs
             raise FloatingPointError("EI is NaN for every candidate (non-finite hyper-parameters or inputs)")
         return out
+
+    # ---- constrained EI (CONS = chooser/GPConstrainedEIChooser.py)
+    def constrained_ei_matrix(self, kind, hyper_samples, chyper_samples, ff, comp, labels, pend, cand, vals,
+                              normals=None):
+        """(M, S) float64 numpy: GPConstrainedEIChooser.ei_over_hypers (CONS:450-468).  Sample PAIRS -- objective sample s
+        with constraint sample s -- are sharded round-robin over ranks, per-sample fantasy normals (S,P,F) with them; the
+        per-candidate sum is all-reduced once (it decides the deep-tail re-evaluation), the disjoint columns once."""
+        eng = self.eng32
+        rank, world = parallel.world()
+        S, M = len(hyper_samples), cand.shape[0]
+        ldm = _ceil(M, 128)
+        mine = parallel.shard(S, rank, world)
+        hs, chs = [hyper_samples[s] for s in mine], [chyper_samples[s] for s in mine]
+        nrm = None if normals is None else np.asarray(normals)[mine]
+        err, ei = None, None
+        ei_sum = torch.zeros((ldm,), dtype=torch.float64, device=eng.device)
+        if hs:
+            try:
+                ei, ei_sum, _ = eng.constrained_ei_over_hypers_device(kind, hs, chs, ff, comp, labels, pend, cand, vals,
+                                                                      nrm)
+            except np.linalg.LinAlgError as e:       # every rank raises, or the others would hang in the all-reduce
+                err = e
+        parallel.agree_on_error(err, eng.device)
+        parallel.allreduce_sum_(ei_sum)
+
+        def rescore(h64, sub):
+            e, s, _ = h64.constrained_ei_over_hypers_device(kind, hs, chs, ff, comp, labels, pend, sub, vals, nrm)
+            return e, s
+        eng.tail_fix(kind, hs, S, comp, pend, cand, vals, nrm, None, None, ei, ei_sum, M,
+                     reduce_fn=parallel.allreduce_sum_, rescore=rescore)
+        if world == 1:
+            return ei[:, :M].t().contiguous().cpu().numpy()
+        full = torch.zeros((S, ldm), dtype=torch.float64, device=eng.device)
+        if ei is not None:
+            full[mine] = ei
+        parallel.allreduce_sum_(full)                # columns are disjoint across ranks
+        return full[:, :M].t().contiguous().cpu().numpy()
+
+    def constraint_predict(self, kind, chyper, ff, comp, cand):
+        """Phi(gain m_c) at ``cand`` for ONE constraint sample (pred_constraint_voilation, CONS:425-447), (M,) numpy."""
+        eng = self.eng32
+        p, _ = eng.constraint_prob_device(kind, [chyper], ff, comp, None, eng.to_dev(cand))
+        return p[0, :cand.shape[0]].cpu().numpy()
+
+    # ---- classification-GP sampler (float64)
+    def latent_loglik(self, kind, comp, ls, noise):
+        """callable(amp2, ff) and .batch([(amp2, ff), ...]): the data term of the joint [amp2, ff] move (CONS:1169-1180)."""
+        return self.eng64.latent_loglik(kind, comp, ls, noise)
+
+    def latent_factor(self, kind, comp, amp2, ls, noise):
+        """.draw(z) = L z, L the lower Cholesky factor of amp2 (k + 1e-6 I) + noise I (CONS:1019-1022, 1193-1200)."""
+        return self.eng64.latent_factor(kind, comp, amp2, ls, noise)
+
+    def constrained_refine_context(self, kind, hyper_samples, chyper_samples, ff, comp, labels, pend, vals,
+                                   normals=None, noise=1e-3):
+        """object with value_grad(x): CONS:471-803 summed over the sample pairs, factors cached."""
+        return self.refine_eng.constrained_refine_context(kind, hyper_samples, chyper_samples, ff, comp, labels, pend,
+                                                          vals, normals, noise)
 
     # ---- f1
     def refine_context(self, kind, hyper_samples, comp, pend, vals, normals=None, time_hyper_samples=None,

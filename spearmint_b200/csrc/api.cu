@@ -66,6 +66,15 @@ template <typename T>
 int ei_sweep(int, int, int, const T*, const T*, int, const T*, const T*, double*, double*, unsigned long long*, cudaStream_t);
 int ei_colsum(int, int, const double*, int, double*, cudaStream_t);
 template <typename T>
+int ei_sweep_weighted(int, int, int, const T*, const T*, int, const T*, const double*, double*, double*,
+                      unsigned long long*, cudaStream_t);
+template <typename T>
+int loglik_set_rhs_batched(int, int, int, const T*, int, T*, cudaStream_t);
+int lower_matvec(int, int, const double*, const double*, double*, cudaStream_t);
+template <typename T>
+int constraint_prob(int, int, int, int, int, int, const T*, const T*, const T*, const T*, const double*, const double*,
+                    double*, double*, int, cudaStream_t);
+template <typename T>
 int topk(int, int, const T*, int*, T*, void*, size_t, cudaStream_t);
 template <typename T>
 int ei_grad_terms(int, int, int, int, int, int, int, const T*, const T*, const T*, const T*, const T*, const T*, T*,
@@ -297,6 +306,37 @@ int smk_ei_sweep_f64(int M, int S, int F, const double* mu, const double* var, i
 }
 int smk_ei_colsum(int M, int S, const double* ei, int ldm, double* ei_sum, void* stream) {
   return ei_colsum(M, S, ei, ldm, ei_sum, ST(stream));
+}
+int smk_ei_sweep_weighted_f32(int M, int S, int F, const float* mu, const float* var, int ldm, const float* best,
+                              const double* w, double* ei, double* ei_sum, unsigned long long* ei_max, void* stream) {
+  return ei_sweep_weighted<float>(M, S, F, mu, var, ldm, best, w, ei, ei_sum, ei_max, ST(stream));
+}
+int smk_ei_sweep_weighted_f64(int M, int S, int F, const double* mu, const double* var, int ldm, const double* best,
+                              const double* w, double* ei, double* ei_sum, unsigned long long* ei_max, void* stream) {
+  return ei_sweep_weighted<double>(M, S, F, mu, var, ldm, best, w, ei, ei_sum, ei_max, ST(stream));
+}
+
+int smk_loglik_set_rhs_batched_f32(int N, int Npad, int S, const float* y, int ldy, float* A, void* stream) {
+  return loglik_set_rhs_batched<float>(N, Npad, S, y, ldy, A, ST(stream));
+}
+int smk_loglik_set_rhs_batched_f64(int N, int Npad, int S, const double* y, int ldy, double* A, void* stream) {
+  return loglik_set_rhs_batched<double>(N, Npad, S, y, ldy, A, ST(stream));
+}
+int smk_lower_matvec_f64(int N, int Npad, const double* L, const double* z, double* out, void* stream) {
+  return lower_matvec(N, Npad, L, z, out, ST(stream));
+}
+
+int smk_constraint_prob_f32(int kind, int N, int Npad, int M, int D, int S, const float* X, const float* C,
+                            const float* inv_ls, const float* amp2, const double* t_alpha, const double* gain,
+                            double* p_out, double* m_out, int ldm, void* stream) {
+  return constraint_prob<float>(kind, N, Npad, M, D, S, X, C, inv_ls, amp2, t_alpha, gain, p_out, m_out, ldm,
+                                ST(stream));
+}
+int smk_constraint_prob_f64(int kind, int N, int Npad, int M, int D, int S, const double* X, const double* C,
+                            const double* inv_ls, const double* amp2, const double* t_alpha, const double* gain,
+                            double* p_out, double* m_out, int ldm, void* stream) {
+  return constraint_prob<double>(kind, N, Npad, M, D, S, X, C, inv_ls, amp2, t_alpha, gain, p_out, m_out, ldm,
+                                 ST(stream));
 }
 
 size_t smk_topk_workspace_bytes(int M, int k) { return topk_workspace_bytes(M, k); }

@@ -162,6 +162,56 @@ template int ei_sweep<float>(int, int, int, const float*, const float*, int, con
 template int ei_sweep<double>(int, int, int, const double*, const double*, int, const double*, const double*,
                               double*, double*, unsigned long long*, cudaStream_t);
 
+// Probability-weighted sweep of the constrained chooser (CONS:878, 940): EI (mean over the F fantasies first) times the
+// probability of feasibility w[s][j] (constraint.cu), otherwise the contract of ei_sweep.  w is double: Phi deep in its
+// tail is far below the float32 range, and so is the product the chooser ranks.
+template <typename T>
+__global__ void __launch_bounds__(256) ei_sweep_weighted_kernel(int M, int S, int F, const T* __restrict__ mu,
+                                                                 const T* __restrict__ var, int ldm,
+                                                                 const T* __restrict__ best, const double* __restrict__ w,
+                                                                 double* __restrict__ ei, double* __restrict__ ei_sum,
+                                                                 unsigned long long* __restrict__ ei_max) {
+  const int j = blockIdx.x * 256 + threadIdx.x;
+  double total = 0.0;
+  for (int s = 0; s < S; ++s) {
+    double e = 0.0;
+    if (j < M) {
+      e = ei_cand<T>(F, mu, var, ldm, best, nullptr, s, j) * w[(long)s * ldm + j];
+      if (ei) ei[(long)s * ldm + j] = e;
+      total += e;
+    }
+    if (ei_max) {
+      double m = (e == e) ? e : 0.0;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+      if ((threadIdx.x & 31) == 0 && m > 0.0) atomicMax(&ei_max[s], (unsigned long long)__double_as_longlong(m));
+    }
+  }
+  if (ei_sum && j < M) ei_sum[j] += total;
+}
+
+template <typename T>
+int ei_sweep_weighted(int M, int S, int F, const T* mu, const T* var, int ldm, const T* best, const double* w, double* ei,
+                      double* ei_sum, unsigned long long* ei_max, cudaStream_t st) {
+  if (M <= 0) return -1;
+  if (S <= 0) return -2;
+  if (F <= 0) return -3;
+  if (!mu) return -4;
+  if (!var) return -5;
+  if (ldm < M) return -6;
+  if (!best) return -7;
+  if (!w) return -8;
+  if (ei_max) cudaMemsetAsync(ei_max, 0, sizeof(unsigned long long) * S, st);
+  ei_sweep_weighted_kernel<T><<<(M + 255) / 256, 256, 0, st>>>(M, S, F, mu, var, ldm, best, w, ei, ei_sum, ei_max);
+  count_launch();
+  return check_launch("ei_sweep_weighted");
+}
+
+template int ei_sweep_weighted<float>(int, int, int, const float*, const float*, int, const float*, const double*,
+                                      double*, double*, unsigned long long*, cudaStream_t);
+template int ei_sweep_weighted<double>(int, int, int, const double*, const double*, int, const double*, const double*,
+                                       double*, double*, unsigned long long*, cudaStream_t);
+
 // ei_sum[j] += sum_s ei[s][j]  (column sum of the per-sample EI matrix; fixed order -> deterministic)
 __global__ void __launch_bounds__(256) ei_colsum_kernel(int M, int S, const double* __restrict__ ei, int ldm,
                                                          double* __restrict__ ei_sum) {

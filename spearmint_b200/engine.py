@@ -28,6 +28,7 @@ from . import _lib
 from ._lib import KINDS, check, fn, ptr
 
 JITTER = 1e-6   # OPT:209-210
+CONSTRAINT_NOISE = 1e-3   # noise of the classification GP of the constrained chooser (CONS:184)
 
 
 def _ceil(x, m):
@@ -485,6 +486,15 @@ class GPEIEngine(object):
                                      ptr(ei_sum) if accumulate else None, ptr(ei_max), self.stream()), "ei_sweep")
         return ei, ei_sum
 
+    def ei_sweep_weighted(self, M, S, F, mu, var, ldm, best, w, want_ei=True, ei_sum=None):
+        """ei_sweep with each per-sample EI multiplied by w[s][j] (double [S][ldm]), CONS:878 / 940."""
+        ei = torch.empty((S, ldm), dtype=torch.float64, device=self.device) if want_ei else None
+        if ei_sum is None:
+            ei_sum = torch.zeros((ldm,), dtype=torch.float64, device=self.device)
+        check(fn("smk_ei_sweep_weighted", self.dtype)(M, S, F, ptr(mu), ptr(var), ldm, ptr(best), ptr(w), ptr(ei),
+                                                      ptr(ei_sum), None, self.stream()), "ei_sweep_weighted")
+        return ei, ei_sum
+
     def topk(self, score, M, k):
         """Indices of the k largest scores, ascending (argsort(score)[-k:], OPT:270; [-1] is the argmax, OPT:294).
         The device selection handles k <= 256 per call; larger k (the reference accepts any grid_subset) takes several
@@ -639,9 +649,10 @@ class GPEIEngine(object):
         p.bests, p.bests_host = self.to_dev(bests), bests
         p.pred_alpha = torch.zeros((S, fac.Npad), dtype=self.dtype, device=self.device)
 
-    def ei_prepared(self, p, Cd, want_matrix=True, ei_sum=None, cand_host=None):
+    def ei_prepared(self, p, Cd, want_matrix=True, ei_sum=None, cand_host=None, weight=None):
         """EI of every candidate in Cd for every sample of a Prepared chunk.  Returns (ei [S][ldm] | None, ei_sum).
-        ``cand_host``: the float64 candidates behind Cd (used only if the accuracy guard re-evaluates a sample)."""
+        ``cand_host``: the float64 candidates behind Cd (used only if the accuracy guard re-evaluates a sample).
+        ``weight``: double [S][ldm] that multiplies each sample's EI (the constrained pass's probability of feasibility)."""
         kind, fac, hb = p.kind, p.fac, p.hb
         M = Cd.shape[0]
         ldm = _ceil(M, 128)
@@ -665,6 +676,12 @@ class GPEIEngine(object):
         self._t1("predict", t)
         t = self._t0()
         guarded = p.gbound is not None and p.host.get("comp") is not None
+        if weight is not None:
+            if guarded or log_time is not None:
+                raise _lib.SmkError("the probability-weighted sweep has no accuracy guard and no per-second variant")
+            out = self.ei_sweep_weighted(M, hb.S, p.F, mu, var, ldm, p.bests, weight, want_matrix, ei_sum)
+            self._t1("ei_sweep", t)
+            return out
         if not guarded:
             out = self.ei_sweep(M, hb.S, p.F, mu, var, ldm, p.bests, log_time, want_matrix, ei_sum)
             self._t1("ei_sweep", t)
@@ -829,14 +846,15 @@ class GPEIEngine(object):
     TAIL_SHORTLIST = 256
 
     def tail_fix(self, kind, hs_local, S_total, comp, pend, cand, vals, normals, ths_local, durs_log, ei, ei_sum, M,
-                 reduce_fn=None):
+                 reduce_fn=None, rescore=None):
         """Late in a run max EI is 1e-8 ... 1e-60: EI = s (u Phi(u) + phi(u)) depends exponentially on u = (best - mu) / s,
         and float32 predictive moments then carry tens of percent of relative error -- enough to reorder the top of the
         ranking, while the reference (float64) proposes its exact argmax (OPT:294).  When the largest mean EI of a pass is
         below TAIL_MEAN_EI, the TAIL_SHORTLIST best candidates of the float32 ranking are re-evaluated with the float64
         build of the same kernels and their EI (per sample and summed) replaces the float32 values, so the argmax / top-k
         are decided in float64 exactly like the reference's.  ``ei_sum`` must already be the global (all-reduced) sum;
-        ``reduce_fn`` all-reduces the short-list sums in place when hyper-samples are sharded over ranks."""
+        ``reduce_fn`` all-reduces the short-list sums in place when hyper-samples are sharded over ranks.
+        ``rescore(h64, cand_sub)`` -> (ei, ei_sum) replaces the plain EI pass of the short-list (constrained EI)."""
         if self.dtype != torch.float32:
             return False
         top = float(ei_sum[:M].max())                       # one scalar read; the caller synchronises right after anyway
@@ -848,8 +866,12 @@ class GPEIEngine(object):
         sub = torch.zeros((k,), dtype=torch.float64, device=self.device)
         if hs_local:
             h64 = self.helper64()
-            e64, s64, _ = h64.ei_over_hypers_device(kind, hs_local, comp, pend, np.ascontiguousarray(cand[idx_h]), vals,
-                                                    normals, ths_local, durs_log, want_matrix=True)
+            sub_cand = np.ascontiguousarray(cand[idx_h])
+            if rescore is not None:
+                e64, s64 = rescore(h64, sub_cand)
+            else:
+                e64, s64, _ = h64.ei_over_hypers_device(kind, hs_local, comp, pend, sub_cand, vals, normals, ths_local,
+                                                        durs_log, want_matrix=True)
             sub += s64[:k]
             if ei is not None:
                 ei[:, idx.long()] = e64[:, :k]
@@ -858,9 +880,121 @@ class GPEIEngine(object):
         ei_sum[idx.long()] = sub
         return True
 
+    # ------------------------------------------------------------------ constrained EI (CONS = GPConstrainedEIChooser.py)
+    def constraint_prob_device(self, kind, chyper_samples, ff, comp, labels, Cd, noise=CONSTRAINT_NOISE, want_mean=False):
+        """P(feasible) = Phi(gain_s m_c(x)) at the candidates Cd, double [S][ldm] (CONS:816-842); with ``want_mean`` also
+        m_c (double [S][ldm], None in the vanilla case).
+
+        ``chyper_samples``: the reference's (constraint_mean, gain, amp2, ls) tuples; ``ff``: the one latent vector over
+        every complete input ``comp`` (violations included) that the reference uses for every sample (CONS:293, 819-839).
+        Without both feasible and violating points the reference skips the classification GP and weights every candidate
+        by Phi(gain_s * 1) (CONS:816-817, 842); ``labels=None`` always evaluates the classification GP
+        (pred_constraint_voilation, CONS:425-447, has no such branch).  Otherwise t_alpha = K_c^-1 ff comes from a FLOAT64
+        factor of amp2 (k + 1e-6 I) + noise I: with noise 1e-3 its entries are large and of both signs, so float32 would lose
+        m_c.  That solve keeps its right-hand side in shared memory (Factor.solve), which limits N to about 14 000
+        complete observations; larger N raises SmkError."""
+        S, M = len(chyper_samples), Cd.shape[0]
+        ldm = _ceil(M, 128)
+        gain = np.array([float(c[1]) for c in chyper_samples])
+        if labels is not None and (np.all(np.asarray(labels) > 0) or np.all(np.asarray(labels) <= 0)):
+            p = torch.as_tensor(sps.norm.cdf(gain), dtype=torch.float64, device=self.device)
+            return p.view(S, 1).expand(S, ldm).contiguous(), None
+        N, D = comp.shape
+        h64 = self.helper64()
+        X64, ff64 = h64.to_dev(comp), h64.to_dev(np.ravel(ff))
+        X = X64 if h64 is self else self.to_dev(comp)
+        gain_d = torch.as_tensor(gain, dtype=torch.float64, device=self.device)
+        p = torch.empty((S, ldm), dtype=torch.float64, device=self.device)
+        m = torch.empty((S, ldm), dtype=torch.float64, device=self.device) if want_mean else None
+        hs = [(0.0, noise, float(c[2]), np.atleast_1d(np.asarray(c[3], dtype=float))) for c in chyper_samples]
+        chunk = h64.max_samples_per_chunk(_ceil(N, 128), ldm)
+        for s0 in range(0, S, chunk):
+            t = self._t0()
+            hb64 = h64.hypers(hs[s0:s0 + chunk], kind)
+            fac = h64.factor(kind, X64, hb64, factor_impl="simt")
+            t_alpha, _, _ = fac.solve(ff64, F=1, subtract_mean=False)           # CONS:834, one ff for every sample
+            self._t1("constraint_factor", t)
+            fac.check_pd()                                                      # LinAlgError like CONS:830
+            hb = hb64 if h64 is self else self.hypers(hs[s0:s0 + chunk], kind)
+            t = self._t0()
+            check(fn("smk_constraint_prob", self.dtype)(KINDS[kind], N, fac.Npad, M, D, hb.S, ptr(X), ptr(Cd),
+                                                        ptr(hb.inv_ls), ptr(hb.amp2), ptr(t_alpha), ptr(gain_d[s0:]),
+                                                        ptr(p[s0:]), ptr(m[s0:]) if want_mean else None, ldm,
+                                                        self.stream()), "constraint_prob")
+            self._t1("constraint_prob", t)
+            del fac
+        return p, m
+
+    def constrained_ei_over_hypers_device(self, kind, hyper_samples, chyper_samples, ff, comp, labels, pend, cand, vals,
+                                          normals=None, noise=CONSTRAINT_NOISE):
+        """The constrained grid pass (CONS:450-468, 806-940) as device tensors: (ei [S][ldm], ei_sum [ldm], M).
+
+        The objective EI is the plain pass on the feasible points only (``labels > 0``), each sample's EI -- mean over the
+        fantasies first -- multiplied by P(feasible) of the paired constraint sample in the same sweep.  ``normals``
+        (S,P,F): the reference draws a fresh fantasy block per sample (CONS:910)."""
+        if self.guard_threshold > 0:
+            raise _lib.SmkError("the constrained pass does not run the tensor-core accuracy guard (SMK_TC_GUARD)")
+        labels = np.asarray(labels)
+        good = labels > 0
+        if not np.any(good):
+            raise ValueError("constrained EI needs at least one feasible observation")
+        comp_g, vals_g = np.ascontiguousarray(comp[good]), np.asarray(vals, dtype=float)[good]
+        S = len(hyper_samples)
+        P = 0 if pend is None else int(pend.shape[0])
+        if len(chyper_samples) != S:
+            raise ValueError("%d objective but %d constraint hyper-samples" % (S, len(chyper_samples)))
+        if np.size(ff) != comp.shape[0]:
+            raise ValueError("ff has %d entries for %d complete observations" % (np.size(ff), comp.shape[0]))
+        if P and (normals is None or np.ndim(normals) != 3 or np.shape(normals)[:2] != (S, P)):
+            raise ValueError("pending points need fantasy normals of shape (S, P, F) = (%d, %d, F), got %s"
+                             % (S, P, None if normals is None else np.shape(normals)))
+        Cd = self.to_dev(cand)
+        M = Cd.shape[0]
+        ldm = _ceil(M, 128)
+        w, _ = self.constraint_prob_device(kind, chyper_samples, ff, comp, labels, Cd, noise)
+        chunk = self.max_samples_per_chunk(_ceil(comp_g.shape[0] + P, 128), ldm, 1 if P == 0 else int(normals.shape[-1]))
+        ei_sum = torch.zeros((ldm,), dtype=torch.float64, device=self.device)
+        ei_all = torch.empty((S, ldm), dtype=torch.float64, device=self.device)
+        for s0 in range(0, S, chunk):
+            nrm = None if normals is None else normals[s0:s0 + chunk]
+            prep = self.prepare(kind, hyper_samples[s0:s0 + chunk], comp_g, pend, vals_g, nrm, cand_dev=Cd)
+            ei, _ = self.ei_prepared(prep, Cd, True, ei_sum, weight=w[s0:s0 + prep.S])
+            prep.fac.check_pd()
+            ei_all[s0:s0 + prep.S] = ei
+            del prep
+        self.last = dict(N=comp.shape[0], N_good=comp_g.shape[0], M=M, S=S, P=P, chunk=chunk)
+        return ei_all, ei_sum, M
+
+    def constrained_ei_over_hypers(self, kind, hyper_samples, chyper_samples, ff, comp, labels, pend, cand, vals,
+                                   normals=None, noise=CONSTRAINT_NOISE):
+        """Host-facing: numpy in, (M,S) float64 numpy out -- GPConstrainedEIChooser.ei_over_hypers (CONS:450-468).
+        In the deep-tail regime the short-list is re-scored by the float64 build (tail_fix)."""
+        ei, ei_sum, M = self.constrained_ei_over_hypers_device(kind, hyper_samples, chyper_samples, ff, comp, labels,
+                                                               pend, cand, vals, normals, noise)
+
+        def rescore(h64, sub):
+            e, s, _ = h64.constrained_ei_over_hypers_device(kind, hyper_samples, chyper_samples, ff, comp, labels, pend,
+                                                            sub, vals, normals, noise)
+            return e, s
+        self.tail_fix(kind, hyper_samples, len(hyper_samples), comp, pend, cand, vals, normals, None, None, ei, ei_sum, M,
+                      rescore=rescore)
+        return ei[:, :M].t().contiguous().cpu().numpy()
+
     # ------------------------------------------------------------------ f2: GP log marginal likelihood
     def loglik(self, kind, comp, vals):
         return LogLik(self, kind, comp, vals)
+
+    # ------------------------------------------------------------------ classification GP of the constrained chooser
+    def latent_loglik(self, kind, comp, ls, noise=CONSTRAINT_NOISE):
+        return LatentLogLik(self, kind, comp, ls, noise)
+
+    def latent_factor(self, kind, comp, amp2, ls, noise):
+        return LatentFactor(self, kind, comp, amp2, ls, noise)
+
+    def constrained_refine_context(self, kind, hyper_samples, chyper_samples, ff, comp, labels, pend, vals, normals=None,
+                                   noise=CONSTRAINT_NOISE):
+        return ConstrainedRefineContext(self, kind, hyper_samples, chyper_samples, ff, comp, labels, pend, vals, normals,
+                                        noise)
 
     # ------------------------------------------------------------------ f1: cached-factor EI value + gradient
     def refine_context(self, kind, hyper_samples, comp, pend, vals, normals=None, time_hyper_samples=None,
@@ -1006,3 +1140,138 @@ class RefineContext(object):
         """Sum over hyper-samples (OPT:360-388)."""
         f_s, g_s = self.per_sample(np.asarray(x, dtype=float))
         return float(f_s.sum()), g_s.sum(axis=0).flatten()
+
+
+# ---------------------------------------------------------------------------------------------- classification GP
+class LatentLogLik(LogLik):
+    """-sum(log diag chol K_c) - 0.5 ff' K_c^-1 ff with K_c = amp2 (k(ls) + 1e-6 I) + noise I: the data term of the joint
+    [amp2, ff] slice move of the constrained chooser (CONS:1169-1180).  ``batch([(amp2, ff), ...])`` evaluates every item
+    with its OWN ff in one batched build + factorisation (smk_loglik_set_rhs_batched puts each ff in its augmented row)."""
+
+    def __init__(self, eng, kind, comp, ls, noise=CONSTRAINT_NOISE, max_batch=None):
+        LogLik.__init__(self, eng, kind, comp, np.zeros(comp.shape[0]), max_batch)
+        self.ls, self.noise = np.atleast_1d(np.asarray(ls, dtype=float)), float(noise)
+
+    def batch(self, items):
+        """items: list of (amp2, ff).  Returns a float64 array; NaN marks a non-PD matrix."""
+        out = np.empty(len(items))
+        eng, dt, N, Npad = self.eng, self.eng.dtype, self.N, self.Npad
+        for b0 in range(0, len(items), self.max_batch):
+            its = items[b0:b0 + self.max_batch]
+            B = len(its)
+            hb = eng.hypers([(0.0, self.noise, float(a), self.ls) for a, _ in its], self.kind)
+            y = eng.to_dev(np.vstack([np.ravel(f) for _, f in its]))
+            st = eng.stream()
+            check(fn("smk_cov_build_lower", dt)(KINDS[self.kind], N, self.D, B, ptr(self.X), ptr(hb.inv_ls),
+                                                ptr(hb.amp2), ptr(hb.noise), ptr(self.L), Npad, st), "cov_build")
+            check(fn("smk_loglik_set_rhs_batched", dt)(N, Npad, B, ptr(y), N, ptr(self.L), st), "loglik_set_rhs_batched")
+            if self.fast:
+                check(_lib.lib().smk_potrf_loglik_f64(Npad, B, ptr(self.L), ptr(self.winv), self.ws_bytes, ptr(self.info),
+                                                      self.use_graph, st), "potrf_loglik")
+            else:
+                check(fn("smk_potrf_lower_batched", dt)(Npad, B, ptr(self.L), ptr(self.winv), ptr(self.info), st), "potrf")
+            check(fn("smk_loglik_finish", dt)(N, Npad, B, ptr(self.L), ptr(self.out[0]), ptr(self.out[1]), st),
+                  "loglik_finish")
+            r = torch.cat([self.out[0, :B].double(), self.out[1, :B].double(), self.info[:B].double()]).cpu().numpy()
+            lp = -r[:B] - 0.5 * r[B:2 * B]
+            lp[r[2 * B:] != 0] = np.nan
+            out[b0:b0 + B] = lp
+            self.calls += B
+            self.launch_batches += 1
+        return out
+
+    def __call__(self, amp2, ff):
+        v = self.batch([(amp2, ff)])[0]
+        if np.isnan(v):
+            raise np.linalg.LinAlgError("leading minor of the array is not positive definite")
+        return v
+
+
+class LatentFactor(object):
+    """The float64 lower Cholesky factor L of amp2 (k(ls) + 1e-6 I) + noise I over the complete inputs; ``draw(z)`` = L z
+    on the device (smk_lower_matvec_f64).  The elliptical-slice direction nu = chol' randn (CONS:1241, chol the upper
+    factor) and the prior draw of a fresh latent (CONS:1019-1022, noise 1e-6) are such products."""
+
+    def __init__(self, eng, kind, comp, amp2, ls, noise):
+        if eng.dtype != torch.float64:
+            raise _lib.SmkError("LatentFactor needs the float64 engine")
+        self.eng = eng
+        hb = eng.hypers([(0.0, float(noise), float(amp2), np.atleast_1d(np.asarray(ls, dtype=float)))], kind)
+        self.fac = eng.factor(kind, eng.to_dev(comp), hb, factor_impl="simt")
+        self.fac.check_pd()                                  # LinAlgError like spla.cholesky (CONS:1021, 1197)
+        self.N = comp.shape[0]
+        self.out = torch.empty((self.N,), dtype=torch.float64, device=eng.device)
+
+    def draw(self, z):
+        zd = self.eng.to_dev(np.ravel(z))
+        check(_lib.lib().smk_lower_matvec_f64(self.N, self.fac.Npad, ptr(self.fac.L), ptr(zd), ptr(self.out),
+                                              self.eng.stream()), "lower_matvec")
+        return self.out.cpu().numpy()
+
+
+class ConstrainedRefineContext(RefineContext):
+    """(f, g) of GPConstrainedEIChooser.grad_optimize_ei_over_hypers (CONS:471-501, 521-803) at one point, summed over the
+    (objective, constraint) sample pairs, with every factor cached:
+      * objective mean from the feasible points (CONS:750 / 607-641); variance from ALL complete points without pending
+        points (CONS:751, 782-784) or from feasible + pending with them (CONS:637, 672);
+      * with pending points EI and gradient are SUMMED over the fantasies and u uses best = min(feasible values), not the
+        fantasy bests (CONS:655, 660, 677); the fantasies come from the normals the caller drew after
+        npr.set_state(randomstate) (CONS:618);
+      * P(feasible) = Phi(gain m_c) from the one latent ``ff``; both gradients carry the reference's 1/2 factor
+        (CONS:675, 786, 683, 796); without a mix of labels the objective EI alone (CONS:679-680, 788-789)."""
+
+    def __init__(self, eng, kind, hyper_samples, chyper_samples, ff, comp, labels, pend, vals, normals=None,
+                 noise=CONSTRAINT_NOISE):
+        if kind == "SE":
+            raise AttributeError("module 'spearmint.gp' has no attribute 'grad_SE'")   # getattr(gp, 'grad_SE')
+        self.eng, self.kind, self.evals = eng, kind, 0
+        labels = np.asarray(labels)
+        good = labels > 0
+        comp_g, vals_g = np.ascontiguousarray(comp[good]), np.asarray(vals, dtype=float)[good]
+        self.best = float(np.min(vals_g))
+        self.pending = pend is not None and pend.shape[0] > 0
+        self.vanilla = bool(np.all(labels > 0) or np.all(labels <= 0))
+        self.prep = eng.prepare(kind, hyper_samples, comp_g, pend if self.pending else None, vals_g,
+                                normals if self.pending else None)
+        self.prep.fac.check_pd()
+        self.hb = self.prep.hb
+        if not self.pending:                 # variance from the factor of ALL complete points (CONS:745-746, 782-784)
+            Xf = eng.to_dev(comp)
+            self.fac_full = eng.factor(kind, Xf, self.hb)
+            self.fac_full.check_pd()
+            self.zero_alpha = torch.zeros((self.hb.S, 1, self.fac_full.Npad), dtype=eng.dtype, device=eng.device)
+        if not self.vanilla:
+            hs = [(0.0, noise, float(c[2]), np.atleast_1d(np.asarray(c[3], dtype=float))) for c in chyper_samples]
+            self.gain = np.array([float(c[1]) for c in chyper_samples])
+            self.camp2 = np.array([float(c[2]) for c in chyper_samples])
+            self.fac_c = eng.factor(kind, eng.to_dev(comp), eng.hypers(hs, kind))
+            self.fac_c.check_pd()                                                # CONS:561, 724
+            self.t_alpha, _, _ = self.fac_c.solve(eng.to_dev(np.ravel(ff)), F=1, subtract_mean=False)
+
+    def per_sample(self, x):
+        p, hb = self.prep, self.hb
+        F, D = p.F, p.fac.D
+        amp2, mean = hb.host_amp2, hb.host_mean
+        out = self._terms(p.fac, p.alpha, F, x)                        # (S, F+1, D+1)
+        m = out[:, :F, D] + mean[:, None]                              # func_m (S,F)
+        gx_m = out[:, :F, :D]
+        if self.pending:
+            v, gx_v = amp2 * (1 + JITTER) - out[:, F, D], -2.0 * out[:, F, :D]
+        else:
+            full = self._terms(self.fac_full, self.zero_alpha, 1, x)
+            v, gx_v = amp2 * (1 + JITTER) - full[:, 1, D], -2.0 * full[:, 1, :D]
+        s = np.sqrt(v)[:, None]
+        u = (self.best - m) / s
+        cdf, pdf = sps.norm.cdf(u), sps.norm.pdf(u)
+        ei = s * (u * cdf + pdf)                                       # (S,F)
+        g_m, g_s2 = -cdf, 0.5 * pdf / s
+        g = 0.5 * amp2[:, None] * (gx_m * g_m[:, :, None] + gx_v[:, None, :] * g_s2[:, :, None]).sum(axis=1)   # (S,D)
+        ei_tot = ei.sum(axis=1)
+        self.evals += 1
+        if self.vanilla:
+            return -ei_tot, g
+        c = self._terms(self.fac_c, self.t_alpha, 1, x)                # (S, 2, D+1)
+        mc = c[:, 0, D]
+        pc = sps.norm.cdf(self.gain * mc)
+        gc = 0.5 * self.camp2[:, None] * self.gain[:, None] * c[:, 0, :D] * sps.norm.pdf(self.gain * mc)[:, None]
+        return -ei_tot * pc, pc[:, None] * g + ei_tot[:, None] * gc
