@@ -70,8 +70,10 @@ int smk_cov_build_lower_f64(int kind, int N, int D, int S, const double* X, cons
                             const double* diag_add, double* out, int ld, void* stream);
 
 /* ---- (2) batched lower Cholesky: spla.cholesky(., lower=True)  (OPT:540, 567, 585)
- * A: [S][Npad][Npad] in/out (lower triangle is read and overwritten with L; the strict upper
- * triangle is left untouched).  winv: [S][Npad/NB][NB][NB] receives the inverses of the
+ * A: [S][Npad][Npad] in/out: only the lower triangle is read, and it is overwritten with L.  On
+ * return the strict upper triangle is unspecified: the trailing updates rewrite the upper half
+ * of the diagonal tiles they touch (and the tensor-core variant below also the block right of
+ * the diagonal in every block-column pair).  winv: [S][Npad/NB][NB][NB] receives the inverses of the
  * diagonal blocks of L (used by every triangular solve below).  info[s] = 0, or 1+index of
  * the first non-positive pivot (the reference raises LinAlgError there, SURVEY 8b).           */
 int smk_potrf_lower_batched_f32(int Npad, int S, float* A, float* winv, int* info, void* stream);
@@ -144,7 +146,8 @@ int smk_tc_np(int N);
 size_t smk_trtri_workspace_bytes(int Np, int S);
 int smk_trtri_split_f32(int Npad, int Np, int S, const float* L, const float* winv, float* linv_hi,
                         float* linv_lo, void* workspace, size_t workspace_bytes, void* stream);
-/* Tensor-core variants of the N^3 steps (float32, 3xTF32, same outputs):
+/* Tensor-core variants of the N^3 steps (float32, 3xTF32; the same outputs, and for the factorisation the same contract
+ * as (2): only the lower triangle of A is read, the strict upper triangle is unspecified on return):
  *   smk_potrf_lower_batched_tc_f32 : left-looking blocked Cholesky, the rank-(jb*128) update of every block-column pair
  *       runs on wgmma (workspace: 2*S*Npad*Npad floats for the tf32 hi/lo copies of the finished panels).
  *   smk_trtri_split_tc_f32 : L^-1 by row blocks, X[K,:] = -(W_KK L[K,:]) X on wgmma; writes linv_hi/linv_lo like

@@ -21,6 +21,7 @@ import pytest
 import scipy.linalg as spla
 
 from oracle import gp_oracle as O
+from tests.helpers import check_rows, ratio, sym
 
 gpu = pytest.mark.gpu
 
@@ -112,46 +113,13 @@ def _same_lower(a, b):
 
 
 # ---------------------------------------------------------------------------------------------------- host references
-def _sym(A):
-    """The symmetric matrix whose lower triangle is A's."""
-    return np.tril(A) + np.tril(A, -1).T
-
-
-def _ratio(L, A, rows):
-    """Componentwise backward error of a Cholesky factor over the lower triangle of the given rows:
-        max_{i in rows, j <= i}  |L L^T - A|_ij / (u (|L| |L|^T)_ij).
-    Componentwise because the augmented pivot A[N, N] = 1e30 would make a normwise max(|L||L^T|) blind to every other
-    entry.  |L L^T - A| <= gamma_{n+1} |L||L^T| holds for Cholesky in any summation order, so LAPACK stays below ~n.
-    An entry whose |L||L^T| is exactly 0 (padding) must be reproduced exactly."""
-    Lr = L[rows]
-    E = np.abs(Lr.dot(L.T) - A[rows])
-    Dn = np.abs(Lr).dot(np.abs(L).T)
-    low = np.arange(A.shape[1])[None, :] <= rows[:, None]
-    if np.any(low & (Dn == 0) & (E != 0)) or not np.all(np.isfinite(E[low])):
-        return np.inf
-    m = low & (Dn > 0)
-    return float((E[m] / Dn[m]).max() / U)
-
-
-def _check_rows(N, Npad, rs):
-    """Rows the backward error is evaluated on when a dense |L||L^T| costs too much on the host: every block's first and
-    last row, every 32-piece boundary of a few blocks, the last 200 rows, row N and 300 random rows."""
-    nblk = Npad // NB
-    r = {b * NB for b in range(nblk)} | {b * NB + NB - 1 for b in range(nblk)}
-    for b in {0, 1, nblk // 2, nblk - 2, nblk - 1}:
-        r |= {b * NB + 32 * p + o for p in range(NB // 32) for o in (0, 31)}
-    r |= set(range(Npad - 200, Npad)) | {N}
-    r |= set(rs.choice(Npad, 300, replace=False).tolist())
-    return np.array(sorted(r))
-
-
 def _kappa(K, N, Lk=None):
     """Spectral condition number of the N x N covariance K (lower triangle read).  At N > 4096 the eigen-decomposition
     costs too much on the host: LAPACK's 1-norm estimate from the factor Lk (kappa_1 >= kappa_2 for a symmetric matrix)."""
     if N <= 4096:
         w = np.linalg.eigvalsh(K[:N, :N])
         return float(w[-1] / w[0])
-    anorm = np.abs(_sym(K[:N, :N])).sum(axis=0).max()
+    anorm = np.abs(sym(K[:N, :N])).sum(axis=0).max()
     rcond, info = spla.lapack.dpocon(Lk[:N, :N], anorm, uplo="L")
     assert info == 0
     return float(1.0 / rcond)
@@ -187,11 +155,11 @@ def _factor_case(eng, record_property, N, kind, D, noise, S, seed, dense):
     sld, quad = _finish(eng, A, N)
 
     # against LAPACK and the oracle, on the host
-    rows = np.arange(Npad) if dense else _check_rows(N, Npad, rs)
+    rows = np.arange(Npad) if dense else check_rows(N, Npad, rs)
     for s, h in enumerate(hs):
         Ah, L = A_in[s].cpu().numpy(), np.tril(A[s].cpu().numpy())
-        Lref = spla.cholesky(_sym(Ah), lower=True, check_finite=False)
-        r_gpu, r_lap = _ratio(L, Ah, rows), _ratio(Lref, Ah, rows)
+        Lref = spla.cholesky(sym(Ah), lower=True, check_finite=False)
+        r_gpu, r_lap = ratio(L, Ah, rows, U), ratio(Lref, Ah, rows, U)
         bound = max(32.0 * r_lap, 2.0 * N)
         record_property("s%d_backward_ratio_gpu" % s, r_gpu)
         record_property("s%d_backward_ratio_lapack" % s, r_lap)
@@ -339,8 +307,8 @@ def test_graph_cache_rollover(eng):
         assert _same_lower(got, ref), "key %d (Npad %d, S %d)" % (k, Npad, S)
         L = np.tril(got[0].cpu().numpy())
         h = inp[0].cpu().numpy()
-        assert _ratio(L, h, np.arange(Npad)) <= max(32.0 * _ratio(spla.cholesky(h, lower=True), h, np.arange(Npad)),
-                                                   2.0 * Npad)
+        assert ratio(L, h, np.arange(Npad), U) <= max(32.0 * ratio(spla.cholesky(h, lower=True), h, np.arange(Npad), U),
+                                                      2.0 * Npad)
 
     for k in range(keys):
         run(k)
