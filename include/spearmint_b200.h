@@ -135,8 +135,13 @@ int smk_predict_f64(int kind, int N, int Npad, int M, int D, int S, const double
  *                         and the round-to-nearest fp16 (hi, lo) pair, each [S][Np][Np] halves.
  *                         linv_exp: [2*S] ints (first S: exponents, rest scratch).
  *   smk_predict_tc_f32  : cross-covariance (candidate-major, fp16 hi/lo) -> D = Kxt * Linv^T on wgmma -> var, mu.
+ *                         var can come out NEGATIVE for a candidate on or next to an observation when the noise is
+ *                         small: beta is formed with the explicit float32 inverse, and |beta|^2 can exceed amp2 (1 + 1e-6)
+ *                         by the inverse's error (measured down to -2.9e-4 amp2 at noise 1e-4, N <= 2560).
+ *                         smk_ei_sweep_* take EI = max(best - mu, 0) wherever var <= 0.
  * alpha: [S][Npad_alpha] (first right-hand side).  dbg_beta (tests only, may be NULL): [S][Mc][Np] dump of
- * beta^T for a single-chunk call.
+ * beta^T, Mc = the candidates of one chunk (ceil128(M) when all fit in one).  Every chunk writes its rows from row 0
+ * of the dump, so after a call of several chunks it holds the last chunk only.
  * z (may be NULL): [S][Np], z = Linv (y - mean) -- the `tmp` output of smk_linv_alpha_f32.  With z the predictive mean is
  *   reduced in the GEMM epilogue (mu - mean = alpha . kx = z . beta) and the generator needs no alpha; then chunk 0 of the
  *   cross-covariance can be generated AHEAD of this call, while K is still being factored:

@@ -1,4 +1,5 @@
-"""Shared helpers of the tests: golden fixture loading, and the host-side measures of a factorisation's error."""
+"""Shared helpers of the tests: golden fixture loading, the inputs of the EI grid pass built as Factor builds them, and
+the host-side measures of a factorisation's error."""
 import os
 
 import numpy as np
@@ -56,6 +57,84 @@ def ratio(L, A, rows, u, R=None):
         return np.inf
     m = low & (Dn > 0)
     return float((E[m] / Dn[m]).max() / u)
+
+
+def data(N, D, seed):
+    """Observations X [N][D] in the unit cube, standardised values y, and the RandomState that drew them."""
+    rs = np.random.RandomState(seed)
+    X = rs.rand(N, D)
+    y = np.sin(3 * X).sum(1) + 0.01 * rs.randn(N)
+    return X, (y - y.mean()) / (y.std() if N > 1 else 1.0), rs
+
+
+def synth_hypers(rs, S, D, noise):
+    """bench.synth's hyper-samples with the given noise."""
+    return [(0.1 * rs.randn(), noise, float(np.exp(0.25 * rs.randn())), rs.uniform(0.3, 2.0, D)) for _ in range(S)]
+
+
+def lib():
+    from spearmint_b200 import _lib as L
+    return L.lib()
+
+
+def cur_stream():
+    import ctypes
+    import torch
+    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def cov_inputs(eng, kind, X, hb, Npad):
+    """[S][Npad][Npad] as Factor builds it: smk_cov_build (full symmetric matrix, identity padding)."""
+    import torch
+    from spearmint_b200.engine import KINDS, check, fn, ptr
+    N, D = X.shape
+    A = torch.zeros((hb.S, Npad, Npad), dtype=eng.dtype, device=eng.device)
+    check(fn("smk_cov_build", eng.dtype)(KINDS[kind], N, N, D, hb.S, ptr(eng.to_dev(X)), None, ptr(hb.inv_ls),
+                                         ptr(hb.amp2), ptr(hb.noise), ptr(A), Npad, eng.stream()), "cov_build")
+    return A
+
+
+def factor_path(path, A, Np):
+    """Factors A [S][Npad][Npad] in place by one path of the EI grid pass:
+      fused   smk_potrf_trtri_tc_f32 (tensor-core Cholesky and explicit inverse in one pipelined call)
+      two     smk_potrf_lower_batched_tc_f32, then smk_trtri_split_tc_f32
+      simt32  smk_potrf_lower_batched_f32, then smk_trtri_split_f32
+      simt64  smk_potrf_lower_batched_f64 (no inverse).
+    Returns {"info" (host), "winv", and for the paths with an explicit inverse "hi", "lo" ([S][Np][Np])}.  Every output
+    buffer starts as NaN, so an element no kernel writes shows up."""
+    import torch
+    from spearmint_b200.engine import check, fn, ptr
+    L = lib()
+    S, Npad, dt, dev = A.shape[0], A.shape[-1], A.dtype, A.device
+    st = cur_stream()
+    nb = NB if dt == torch.float32 else 64
+    out = {"winv": torch.full((S, Npad // nb, nb, nb), float("nan"), dtype=dt, device=dev)}
+    info = torch.full((S,), -1, dtype=torch.int32, device=dev)
+    if path != "simt64":
+        out["hi"] = torch.full((S, Np, Np), float("nan"), dtype=torch.float32, device=dev)
+        out["lo"] = torch.full((S, Np, Np), float("nan"), dtype=torch.float32, device=dev)
+    if path in ("fused", "two"):
+        nb_p = 2 * S * Npad * Npad * 4
+        ws = torch.empty((nb_p,), dtype=torch.uint8, device=dev)
+        nb_t = L.smk_trtri_tc_workspace_bytes(Npad, Np, S)
+        wt = torch.empty((nb_t,), dtype=torch.uint8, device=dev)
+        if path == "fused":
+            check(L.smk_potrf_trtri_tc_f32(Npad, Np, S, ptr(A), ptr(out["winv"]), ptr(info), ptr(ws), nb_p,
+                                           ptr(out["hi"]), ptr(out["lo"]), ptr(wt), nb_t, st), "potrf_trtri_tc")
+        else:
+            check(L.smk_potrf_lower_batched_tc_f32(Npad, S, ptr(A), ptr(out["winv"]), ptr(info), ptr(ws), nb_p, st),
+                  "potrf_tc")
+            check(L.smk_trtri_split_tc_f32(Npad, Np, S, ptr(A), ptr(out["winv"]), ptr(out["hi"]), ptr(out["lo"]),
+                                           ptr(wt), nb_t, st), "trtri_split_tc")
+    else:
+        check(fn("smk_potrf_lower_batched", dt)(Npad, S, ptr(A), ptr(out["winv"]), ptr(info), st), "potrf")
+        if path == "simt32":
+            nb_t = L.smk_trtri_workspace_bytes(Np, S)
+            wt = torch.empty((nb_t,), dtype=torch.uint8, device=dev)
+            check(L.smk_trtri_split_f32(Npad, Np, S, ptr(A), ptr(out["winv"]), ptr(out["hi"]), ptr(out["lo"]), ptr(wt),
+                                        nb_t, st), "trtri_split")
+    out["info"] = info.cpu().numpy()           # read back: nothing of this call is in flight afterwards
+    return out
 
 
 def check_rows(N, Npad, rs, nb=NB):

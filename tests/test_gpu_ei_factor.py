@@ -28,6 +28,8 @@ import pytest
 import scipy.linalg as spla
 
 from tests.helpers import check_rows, ratio, sym
+from tests.helpers import cov_inputs as _inputs, cur_stream as _stream, data as _data, factor_path as _factor
+from tests.helpers import lib as _lib, synth_hypers as _hypers
 
 gpu = pytest.mark.gpu
 
@@ -51,78 +53,6 @@ def engs():
     import torch
     from spearmint_b200.engine import GPEIEngine
     return {"f32": GPEIEngine(dtype=torch.float32), "f64": GPEIEngine(dtype=torch.float64)}
-
-
-def _lib():
-    from spearmint_b200 import _lib as L
-    return L.lib()
-
-
-def _stream():
-    import ctypes
-    import torch
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _data(N, D, seed):
-    rs = np.random.RandomState(seed)
-    X = rs.rand(N, D)
-    y = np.sin(3 * X).sum(1) + 0.01 * rs.randn(N)
-    return X, (y - y.mean()) / (y.std() if N > 1 else 1.0), rs
-
-
-def _hypers(rs, S, D, noise):
-    """bench.synth's hyper-samples with the given noise."""
-    return [(0.1 * rs.randn(), noise, float(np.exp(0.25 * rs.randn())), rs.uniform(0.3, 2.0, D)) for _ in range(S)]
-
-
-def _inputs(eng, kind, X, hb, Npad):
-    """[S][Npad][Npad] as Factor builds it: smk_cov_build (full symmetric matrix, identity padding)."""
-    import torch
-    from spearmint_b200.engine import KINDS, check, fn, ptr
-    N, D = X.shape
-    A = torch.zeros((hb.S, Npad, Npad), dtype=eng.dtype, device=eng.device)
-    check(fn("smk_cov_build", eng.dtype)(KINDS[kind], N, N, D, hb.S, ptr(eng.to_dev(X)), None, ptr(hb.inv_ls),
-                                         ptr(hb.amp2), ptr(hb.noise), ptr(A), Npad, eng.stream()), "cov_build")
-    return A
-
-
-def _factor(path, A, Np):
-    """Factors A [S][Npad][Npad] in place by one path.  Returns {"info" (host), "winv", and for the paths with an explicit
-    inverse "hi", "lo" ([S][Np][Np])}.  Every output buffer starts as NaN, so an element no kernel writes shows up."""
-    import torch
-    from spearmint_b200.engine import check, fn, ptr
-    L = _lib()
-    S, Npad, dt, dev = A.shape[0], A.shape[-1], A.dtype, A.device
-    st = _stream()
-    nb = NB if dt == torch.float32 else NB64
-    out = {"winv": torch.full((S, Npad // nb, nb, nb), float("nan"), dtype=dt, device=dev)}
-    info = torch.full((S,), -1, dtype=torch.int32, device=dev)
-    if path != "simt64":
-        out["hi"] = torch.full((S, Np, Np), float("nan"), dtype=torch.float32, device=dev)
-        out["lo"] = torch.full((S, Np, Np), float("nan"), dtype=torch.float32, device=dev)
-    if path in ("fused", "two"):
-        nb_p = 2 * S * Npad * Npad * 4
-        ws = torch.empty((nb_p,), dtype=torch.uint8, device=dev)
-        nb_t = L.smk_trtri_tc_workspace_bytes(Npad, Np, S)
-        wt = torch.empty((nb_t,), dtype=torch.uint8, device=dev)
-        if path == "fused":
-            check(L.smk_potrf_trtri_tc_f32(Npad, Np, S, ptr(A), ptr(out["winv"]), ptr(info), ptr(ws), nb_p,
-                                           ptr(out["hi"]), ptr(out["lo"]), ptr(wt), nb_t, st), "potrf_trtri_tc")
-        else:
-            check(L.smk_potrf_lower_batched_tc_f32(Npad, S, ptr(A), ptr(out["winv"]), ptr(info), ptr(ws), nb_p, st),
-                  "potrf_tc")
-            check(L.smk_trtri_split_tc_f32(Npad, Np, S, ptr(A), ptr(out["winv"]), ptr(out["hi"]), ptr(out["lo"]),
-                                           ptr(wt), nb_t, st), "trtri_split_tc")
-    else:
-        check(fn("smk_potrf_lower_batched", dt)(Npad, S, ptr(A), ptr(out["winv"]), ptr(info), st), "potrf")
-        if path == "simt32":
-            nb_t = L.smk_trtri_workspace_bytes(Np, S)
-            wt = torch.empty((nb_t,), dtype=torch.uint8, device=dev)
-            check(L.smk_trtri_split_f32(Npad, Np, S, ptr(A), ptr(out["winv"]), ptr(out["hi"]), ptr(out["lo"]), ptr(wt),
-                                        nb_t, st), "trtri_split")
-    out["info"] = info.cpu().numpy()           # read back: nothing of this call is in flight afterwards
-    return out
 
 
 def _same(a, b, A, B):
