@@ -81,6 +81,7 @@ for _t in ("f32", "f64"):
         "smk_cov_build_lower_" + _t: ([_i] * 4 + [_p] * 5 + [_i, _p], _i),
         "smk_potrf_lower_batched_" + _t: ([_i, _i, _p, _p, _p, _p], _i),
         "smk_chol_solve_" + _t: ([_i] * 4 + [_p, _p, _p, _ll, _i, _p, _p, _p, _p, _p], _i),
+        "smk_chol_solve_gm_" + _t: ([_i] * 4 + [_p, _p, _p, _ll, _i, _p, _p, _p, _p, _p], _i),
         "smk_loglik_set_rhs_" + _t: ([_i, _i, _i, _p, _p, _p, _p], _i),
         "smk_loglik_finish_" + _t: ([_i, _i, _i, _p, _p, _p, _p], _i),
         "smk_predict_" + _t: ([_i] * 6 + [_p] * 10 + [_i, _p, _sz, _p], _i),

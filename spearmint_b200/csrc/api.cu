@@ -53,6 +53,8 @@ int potrf_lower_batched(int, int, T*, T*, int*, cudaStream_t);
 template <typename T>
 int chol_solve(int, int, int, int, const T*, const T*, const T*, long long, int, const T*, T*, T*, T*, cudaStream_t);
 template <typename T>
+int chol_solve_gm(int, int, int, int, const T*, const T*, const T*, long long, int, const T*, T*, T*, T*, cudaStream_t);
+template <typename T>
 int loglik_set_rhs(int, int, int, const T*, const T*, T*, cudaStream_t);
 template <typename T>
 int loglik_finish(int, int, int, const T*, T*, T*, cudaStream_t);
@@ -183,6 +185,16 @@ int smk_chol_solve_f64(int N, int Npad, int S, int F, const double* L, const dou
                        long long y_stride, int ldy, const double* mean, double* alpha, double* sum_log_diag,
                        double* quad, void* stream) {
   return chol_solve<double>(N, Npad, S, F, L, winv, y, y_stride, ldy, mean, alpha, sum_log_diag, quad, ST(stream));
+}
+int smk_chol_solve_gm_f32(int N, int Npad, int S, int F, const float* L, const float* winv, const float* y,
+                          long long y_stride, int ldy, const float* mean, float* alpha, float* sum_log_diag,
+                          float* quad, void* stream) {
+  return chol_solve_gm<float>(N, Npad, S, F, L, winv, y, y_stride, ldy, mean, alpha, sum_log_diag, quad, ST(stream));
+}
+int smk_chol_solve_gm_f64(int N, int Npad, int S, int F, const double* L, const double* winv, const double* y,
+                          long long y_stride, int ldy, const double* mean, double* alpha, double* sum_log_diag,
+                          double* quad, void* stream) {
+  return chol_solve_gm<double>(N, Npad, S, F, L, winv, y, y_stride, ldy, mean, alpha, sum_log_diag, quad, ST(stream));
 }
 
 int smk_loglik_set_rhs_f32(int N, int Npad, int S, const float* y, const float* mean, float* A, void* stream) {

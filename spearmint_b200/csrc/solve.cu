@@ -206,6 +206,266 @@ __global__ void __launch_bounds__(256) chol_solve_kernel(int N, int Npad, int F,
       if (f0 + r < F) alpha[((long)s * F + f0 + r) * Npad + n] = x[r * Npad + n];
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// The same solve with the right-hand sides in global memory (alpha is the working vector), for any Npad.
+// Right-looking in both directions, one launch per block step; L is read once per direction by the whole grid.
+// A CTA owns (one FB-group of right-hand sides, one target tile, one sample); it forms the step's diagonal-block
+// product t = W x redundantly (NB^2 per right-hand side) and applies it to its own tile:
+//   forward, step J:   x_I -= L_IJ t_J,        t_J = W_JJ x_J,     every block row I > J
+//   backward, step I:  x_J -= L_IJ^T a_I,      a_I = W_II^T x_I,   every block column J < I
+// The CTAs of step J all read x_J, so none of them may overwrite it: CTA 0 of the NEXT launch forms the same product
+// again and stores it (no other CTA of that launch touches that block).  Only rows < N are read or written: under
+// n_lead < N the rows >= N of L and winv belong to a larger joint factor and may hold anything, and alpha keeps zeros
+// there from the initialisation.
+template <typename T>
+__global__ void solve_gm_init_kernel(int N, int Npad, int F, const T* __restrict__ y, long long y_stride, int ldy,
+                                     const T* __restrict__ mean, T* __restrict__ x, long long total) {
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const long long sf = e / Npad;
+    const int n = (int)(e - sf * Npad);
+    const long long s = sf / F;
+    const int f = (int)(sf - s * F);
+    x[e] = n < N ? y[s * y_stride + (long long)f * ldy + n] - (mean ? mean[s] : T(0)) : T(0);
+  }
+}
+
+// xs[r][k] = x[s][f0+r][base+k] for rows < N and f < F, else 0
+template <typename T, int FB>
+__device__ __forceinline__ void solve_gm_load(T (*xs)[Cfg<T>::NB], const T* x, int N, int Npad, int F, int f0, int base) {
+  constexpr int NB = Cfg<T>::NB;
+  for (int e = threadIdx.x; e < FB * NB; e += 256) {
+    const int r = e / NB, k = e % NB;
+    xs[r][k] = (f0 + r < F && base + k < N) ? x[(long long)(f0 + r) * Npad + base + k] : T(0);
+  }
+}
+
+template <typename T, int FB>
+__device__ __forceinline__ void solve_gm_store(const T (*ts)[Cfg<T>::NB], T* x, int N, int Npad, int F, int f0, int base) {
+  constexpr int NB = Cfg<T>::NB;
+  for (int e = threadIdx.x; e < FB * NB; e += 256) {
+    const int r = e / NB, k = e % NB;
+    if (f0 + r < F && base + k < N) x[(long long)(f0 + r) * Npad + base + k] = ts[r][k];
+  }
+}
+
+// Forward step J (launch J = 0 .. nbN): blockIdx.y == 0 stores t_{J-1} into x_{J-1}; blockIdx.y = b > 0 updates block
+// row I = J + b with t_J.  Rows of a tile are dotted by one warp, four at a time, lanes along the contiguous columns.
+template <typename T, int FB>
+__global__ void __launch_bounds__(256) solve_gm_fwd_kernel(int N, int Npad, int F, int J, const T* __restrict__ L,
+                                                           const T* __restrict__ winv, T* __restrict__ x) {
+  constexpr int NB = Cfg<T>::NB;
+  __shared__ T xs[FB][NB], ts[FB][NB];
+  const bool store = blockIdx.y == 0;
+  const int K = store ? J - 1 : J;
+  if (K < 0) return;
+  const int f0 = blockIdx.x * FB, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const long long s = blockIdx.z;
+  const T* Ls = L + s * Npad * (long long)Npad;
+  const T* Wb = winv + (s * (Npad / NB) + K) * (long long)(NB * NB);
+  T* xs_g = x + s * F * (long long)Npad;
+  const int base = K * NB;
+  solve_gm_load<T, FB>(xs, xs_g, N, Npad, F, f0, base);
+  __syncthreads();
+  // t[i] = sum_{k <= i} W[i][k] x[k], rows i < N
+  for (int i0 = warp * 4; i0 < NB; i0 += 32) {
+    T p[4][FB];
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+#pragma unroll
+      for (int r = 0; r < FB; ++r) p[q][r] = T(0);
+    for (int k = lane; k < NB; k += 32) {
+      T w[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) w[q] = (k <= i0 + q && base + i0 + q < N) ? Wb[(i0 + q) * NB + k] : T(0);
+#pragma unroll
+      for (int r = 0; r < FB; ++r) {
+        const T xv = xs[r][k];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) p[q][r] = fma(w[q], xv, p[q][r]);
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+#pragma unroll
+      for (int r = 0; r < FB; ++r) {
+        const T v = warp_sum(p[q][r]);
+        if (lane == 0) ts[r][i0 + q] = v;
+      }
+  }
+  __syncthreads();
+  if (store) {
+    solve_gm_store<T, FB>(ts, xs_g, N, Npad, F, f0, base);
+    return;
+  }
+  // x_I[i] -= sum_k L[I*NB + i][base + k] t[k], rows < N (columns base + k < I*NB are then < N too)
+  const int rbase = (J + blockIdx.y) * NB;
+  for (int i0 = warp * 4; i0 < NB; i0 += 32) {
+    T p[4][FB];
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+#pragma unroll
+      for (int r = 0; r < FB; ++r) p[q][r] = T(0);
+    for (int k = lane; k < NB; k += 32) {
+      T l[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        l[q] = rbase + i0 + q < N ? Ls[(long long)(rbase + i0 + q) * Npad + base + k] : T(0);
+#pragma unroll
+      for (int r = 0; r < FB; ++r) {
+        const T tv = ts[r][k];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) p[q][r] = fma(l[q], tv, p[q][r]);
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+#pragma unroll
+      for (int r = 0; r < FB; ++r) {
+        const T v = warp_sum(p[q][r]);
+        const int row = rbase + i0 + q;
+        if (lane == ((q * FB + r) & 31) && row < N && f0 + r < F) xs_g[(long long)(f0 + r) * Npad + row] -= v;
+      }
+  }
+}
+
+// Backward step I (launch I = nbN-1 .. -1): blockIdx.y == 0 stores a_{I+1} into x_{I+1}; blockIdx.y = b > 0 updates
+// block column J = b - 1 < I with a_I.  A thread owns one column and walks rows in NG interleaved groups (coalesced
+// row reads of W and L); the groups are summed in a fixed order.
+template <typename T, int FB>
+__global__ void __launch_bounds__(256) solve_gm_bwd_kernel(int N, int Npad, int F, int I, int nbN,
+                                                           const T* __restrict__ L, const T* __restrict__ winv,
+                                                           T* __restrict__ x) {
+  constexpr int NB = Cfg<T>::NB, NG = 256 / NB;
+  __shared__ T xs[FB][NB], ts[FB][NB], red[NG][FB][NB];
+  const bool store = blockIdx.y == 0;
+  const int K = store ? I + 1 : I;
+  if (K < 0 || K >= nbN) return;
+  const int f0 = blockIdx.x * FB, tid = threadIdx.x, c = tid % NB, g = tid / NB;
+  const long long s = blockIdx.z;
+  const T* Ls = L + s * Npad * (long long)Npad;
+  const T* Wb = winv + (s * (Npad / NB) + K) * (long long)(NB * NB);
+  T* xs_g = x + s * F * (long long)Npad;
+  const int base = K * NB;
+  solve_gm_load<T, FB>(xs, xs_g, N, Npad, F, f0, base);
+  __syncthreads();
+  // a[c] = sum_{c <= k, base + k < N} W[k][c] x[k]
+  T p[FB];
+#pragma unroll
+  for (int r = 0; r < FB; ++r) p[r] = T(0);
+  for (int k = c + g; k < NB && base + k < N; k += NG) {
+    const T w = Wb[k * NB + c];
+#pragma unroll
+    for (int r = 0; r < FB; ++r) p[r] = fma(w, xs[r][k], p[r]);
+  }
+#pragma unroll
+  for (int r = 0; r < FB; ++r) red[g][r][c] = p[r];
+  __syncthreads();
+  for (int e = tid; e < FB * NB; e += 256) {
+    const int r = e / NB, k = e % NB;
+    T v = T(0);
+#pragma unroll
+    for (int gg = 0; gg < NG; ++gg) v += red[gg][r][k];
+    ts[r][k] = v;
+  }
+  __syncthreads();
+  if (store) {
+    solve_gm_store<T, FB>(ts, xs_g, N, Npad, F, f0, base);
+    return;
+  }
+  // x_J[c] -= sum_{i: base + i < N} L[base + i][J*NB + c] a[i]
+  const int cbase = (blockIdx.y - 1) * NB;
+#pragma unroll
+  for (int r = 0; r < FB; ++r) p[r] = T(0);
+  for (int i = g; i < NB && base + i < N; i += NG) {
+    const T l = Ls[(long long)(base + i) * Npad + cbase + c];
+#pragma unroll
+    for (int r = 0; r < FB; ++r) p[r] = fma(l, ts[r][i], p[r]);
+  }
+#pragma unroll
+  for (int r = 0; r < FB; ++r) red[g][r][c] = p[r];
+  __syncthreads();
+  for (int e = tid; e < FB * NB; e += 256) {
+    const int r = e / NB, k = e % NB;
+    if (f0 + r >= F) continue;
+    T v = T(0);
+#pragma unroll
+    for (int gg = 0; gg < NG; ++gg) v += red[gg][r][k];
+    xs_g[(long long)(f0 + r) * Npad + cbase + k] -= v;
+  }
+}
+
+// quad[s][f] = |x[s][f]|^2 after the forward pass (rows >= N are zero);  sum_log_diag[s] from blockIdx.x == 0
+template <typename T>
+__global__ void __launch_bounds__(256) solve_gm_scalars_kernel(int N, int Npad, int F, const T* __restrict__ L,
+                                                               const T* __restrict__ x, T* __restrict__ sum_log_diag,
+                                                               T* __restrict__ quad) {
+  __shared__ T red8[8];
+  const long long s = blockIdx.y;
+  const int f = blockIdx.x, tid = threadIdx.x;
+  if (quad) {
+    const T* xr = x + (s * F + f) * (long long)Npad;
+    T a = T(0);
+    for (int n = tid; n < N; n += 256) a = fma(xr[n], xr[n], a);
+    a = block_sum(a, red8);
+    if (tid == 0) quad[s * F + f] = a;
+  }
+  if (sum_log_diag && f == 0) {
+    const T* Ls = L + s * Npad * (long long)Npad;
+    T a = T(0);
+    for (int n = tid; n < N; n += 256) a += smk_log(Ls[(long long)n * Npad + n]);
+    a = block_sum(a, red8);
+    if (tid == 0) sum_log_diag[s] = a;
+  }
+}
+
+template <typename T, int FB>
+static void solve_gm_forward(int N, int Npad, int S, int F, const T* L, const T* winv, T* alpha, cudaStream_t st) {
+  constexpr int NB = Cfg<T>::NB;
+  const int nbN = (N + NB - 1) / NB, ng = (F + FB - 1) / FB;
+  for (int J = 0; J <= nbN; ++J)
+    solve_gm_fwd_kernel<T, FB><<<dim3(ng, J < nbN ? nbN - J : 1, S), 256, 0, st>>>(N, Npad, F, J, L, winv, alpha);
+  count_launch(nbN + 1);
+}
+
+template <typename T, int FB>
+static void solve_gm_backward(int N, int Npad, int S, int F, const T* L, const T* winv, T* alpha, cudaStream_t st) {
+  constexpr int NB = Cfg<T>::NB;
+  const int nbN = (N + NB - 1) / NB, ng = (F + FB - 1) / FB;
+  for (int I = nbN - 1; I >= -1; --I)
+    solve_gm_bwd_kernel<T, FB><<<dim3(ng, I + 1 > 0 ? I + 1 : 1, S), 256, 0, st>>>(N, Npad, F, I, nbN, L, winv, alpha);
+  count_launch(nbN + 1);
+}
+
+template <typename T>
+int chol_solve_gm(int N, int Npad, int S, int F, const T* L, const T* winv, const T* y, long long y_stride, int ldy,
+                  const T* mean, T* alpha, T* sum_log_diag, T* quad, cudaStream_t st) {
+  if (N <= 0) return -1;
+  if (Npad < N || Npad % kNpadMult) return -2;
+  if (S <= 0 || S > 65535) return -3;
+  if (F <= 0) return -4;
+  if (!L) return -5;
+  if (!winv) return -6;
+  if (!y) return -7;
+  if (ldy < N) return -9;
+  if (!alpha) return -11;
+  const long long total = (long long)S * F * Npad;
+  const int ib = (int)(total / 256 + 1 < 132 * 16 ? total / 256 + 1 : 132 * 16);
+  solve_gm_init_kernel<T><<<ib, 256, 0, st>>>(N, Npad, F, y, y_stride, ldy, mean, alpha, total);
+  count_launch();
+  // FB right-hand sides per CTA: one when there is one, else a group that reuses each L element 4 or 8 times
+  if (F == 1) solve_gm_forward<T, 1>(N, Npad, S, F, L, winv, alpha, st);
+  else if (F <= 4) solve_gm_forward<T, 4>(N, Npad, S, F, L, winv, alpha, st);
+  else solve_gm_forward<T, 8>(N, Npad, S, F, L, winv, alpha, st);
+  if (quad || sum_log_diag) {
+    solve_gm_scalars_kernel<T><<<dim3(F, S), 256, 0, st>>>(N, Npad, F, L, alpha, sum_log_diag, quad);
+    count_launch();
+  }
+  if (F == 1) solve_gm_backward<T, 1>(N, Npad, S, F, L, winv, alpha, st);
+  else if (F <= 4) solve_gm_backward<T, 4>(N, Npad, S, F, L, winv, alpha, st);
+  else solve_gm_backward<T, 8>(N, Npad, S, F, L, winv, alpha, st);
+  return check_launch("chol_solve_gm");
+}
+
 template <typename T>
 int chol_solve(int N, int Npad, int S, int F, const T* L, const T* winv, const T* y, long long y_stride, int ldy,
                const T* mean, T* alpha, T* sum_log_diag, T* quad, cudaStream_t st) {
@@ -219,7 +479,9 @@ int chol_solve(int N, int Npad, int S, int F, const T* L, const T* winv, const T
   if (!y) return -7;
   if (ldy < N) return -9;
   const size_t dsm = sizeof(T) * ((size_t)RB * Npad + RB * NB + (size_t)NG * RB * NB);
-  if (dsm > 227 * 1024) return -2;
+  // the right-hand sides of one CTA no longer fit in shared memory (next to the kernel's static red8[8])
+  if (dsm + 8 * sizeof(T) > 227 * 1024) return chol_solve_gm<T>(N, Npad, S, F, L, winv, y, y_stride, ldy, mean, alpha, sum_log_diag,
+                                                quad, st);
   static size_t attr_set = 0;
   if (dsm > attr_set) {
     cudaFuncSetAttribute(chol_solve_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dsm);
@@ -291,5 +553,9 @@ template int chol_solve<float>(int, int, int, int, const float*, const float*, c
                                const float*, float*, float*, float*, cudaStream_t);
 template int chol_solve<double>(int, int, int, int, const double*, const double*, const double*, long long, int,
                                 const double*, double*, double*, double*, cudaStream_t);
+template int chol_solve_gm<float>(int, int, int, int, const float*, const float*, const float*, long long, int,
+                                  const float*, float*, float*, float*, cudaStream_t);
+template int chol_solve_gm<double>(int, int, int, int, const double*, const double*, const double*, long long, int,
+                                   const double*, double*, double*, double*, cudaStream_t);
 
 }  // namespace smk

@@ -200,10 +200,6 @@ class Factor(object):
         eng, hb = self.eng, self.hb
         S, dt, dev = hb.S, eng.dtype, eng.device
         n = self.N if n_lead is None else n_lead
-        rb, nb_ = (4, 128) if dt == torch.float32 else (2, 64)
-        if eng.esize * (rb * self.Npad + rb * nb_ + (256 // nb_) * rb * nb_) > 227 * 1024:
-            raise _lib.SmkError("chol_solve keeps its right-hand sides in shared memory: N = %d exceeds its limit (about "
-                                "%d for this element type); use the explicit-inverse path" % (self.N, 227 * 1024 // (eng.esize * rb)))
         alpha = torch.empty((S, F, self.Npad), dtype=dt, device=dev) if want_alpha else None
         sld = torch.empty((S,), dtype=dt, device=dev) if want_logdet else None
         quad = torch.empty((S, F), dtype=dt, device=dev) if want_quad else None
@@ -891,8 +887,8 @@ class GPEIEngine(object):
         by Phi(gain_s * 1) (CONS:816-817, 842); ``labels=None`` always evaluates the classification GP
         (pred_constraint_voilation, CONS:425-447, has no such branch).  Otherwise t_alpha = K_c^-1 ff comes from a FLOAT64
         factor of amp2 (k + 1e-6 I) + noise I: with noise 1e-3 its entries are large and of both signs, so float32 would lose
-        m_c.  That solve keeps its right-hand side in shared memory (Factor.solve), which limits N to about 14 000
-        complete observations; larger N raises SmkError."""
+        m_c.  Past about 14 000 complete observations that solve keeps its right-hand side in global memory
+        (smk_chol_solve_gm_f64), so any N whose factors fit on the device works."""
         S, M = len(chyper_samples), Cd.shape[0]
         ldm = _ceil(M, 128)
         gain = np.array([float(c[1]) for c in chyper_samples])
