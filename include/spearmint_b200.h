@@ -298,7 +298,10 @@ int smk_ei_over_hypers_host_f32(int kind, int N, int M, int D, int S, const doub
  * out: [S][Q][F+1][D+1]:  out[f][d] = sum_n alpha_f[n] gk[n][d];  out[f][D] = kx' alpha_f;
  *                         out[F][d] = sum_n gamma[n] gk[n][d];     out[F][D] = kx' K^-1 kx,
  * with gk[n][d] = dk/dr2 * (2/ls_d) (X[n][d] - xq[d]) / ls_d  (correlation gradient, no amp2 -- the
- * reference applies 0.5*amp2 afterwards, OPT:437).  kind SMK_SE is rejected like the reference (no gp.grad_SE). */
+ * reference applies 0.5*amp2 afterwards, OPT:437).  kind SMK_SE is rejected like the reference (no gp.grad_SE): -1.
+ * Any F >= 1 (the fantasy rows are staged 64 at a time); -4 also when D is too large for the shared-memory staging
+ * (D > 324 in float64, D > 712 in float32).  Each output element is summed over n = 0 .. N-1 in order, so row f of
+ * an F-fantasy call equals row f of any call with more fantasies bit for bit.                                     */
 int smk_ei_grad_terms_f32(int kind, int N, int Npad, int D, int S, int Q, int F, const float* X, const float* xq,
                           const float* inv_ls, const float* amp2, const float* alpha, const float* gamma,
                           float* out, void* stream);

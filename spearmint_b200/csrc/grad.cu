@@ -29,6 +29,10 @@ __device__ __forceinline__ T dk_dr2(int kind, T r2) {
 }
 
 constexpr int kGC = 64;  // rows of X per staged chunk
+constexpr int kFR = 64;  // rows of A (fantasies + the gamma row) staged at a time: shared memory does not grow with F
+
+// Rows of A one pass of pairs reads.
+__host__ __device__ __forceinline__ int ei_grad_rows(int F) { return F + 1 < kFR ? F + 1 : kFR; }
 
 template <typename T>
 __global__ void __launch_bounds__(256) ei_grad_terms_kernel(int kind, int N, int Npad, int D, int Q, int F,
@@ -40,8 +44,8 @@ __global__ void __launch_bounds__(256) ei_grad_terms_kernel(int kind, int N, int
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int D1 = D + 1, F1 = F + 1;
   T* Tt = reinterpret_cast<T*>(smem_raw);   // [kGC][D1]
-  T* At = Tt + kGC * D1;                    // [F1][kGC]
-  T* xs = At + F1 * kGC;                    // [D] scaled query point
+  T* At = Tt + kGC * D1;                    // [ei_grad_rows(F)][kGC]: rows f0 .. f0 + nf - 1 of A
+  T* xs = At + ei_grad_rows(F) * kGC;       // [D] scaled query point
   T* il = xs + D;                           // [D]
   const int q = blockIdx.x, s = blockIdx.y, tid = threadIdx.x;
   for (int d = tid; d < D; d += 256) {
@@ -56,8 +60,13 @@ __global__ void __launch_bounds__(256) ei_grad_terms_kernel(int kind, int N, int
   T* o = out + ((long)s * Q + q) * F1 * D1;
   const int npairs = F1 * D1;
   constexpr int R = 8;
+  // pairs (f, d), p = f D1 + d, in passes of up to 256 R; a pass of at most (kFR - 1) D1 + 1 pairs reads at most kFR
+  // rows of A.  Each output element is one pass's sum over n = 0 .. N-1 in order, whatever the pass boundaries.
+  const int P = F1 <= kFR ? 256 * R : min(256 * R, (kFR - 1) * D1);
 
-  for (int p0 = 0; p0 < npairs; p0 += 256 * R) {
+  for (int p0 = 0; p0 < npairs; p0 += P) {
+    const int p1 = min(npairs, p0 + P);
+    const int f0 = p0 / D1, nf = (p1 - 1) / D1 - f0 + 1;
     T acc[R];
 #pragma unroll
     for (int r = 0; r < R; ++r) acc[r] = T(0);
@@ -86,16 +95,16 @@ __global__ void __launch_bounds__(256) ei_grad_terms_kernel(int kind, int N, int
         Tt[i * D1 + d] = g;
       }
       __syncthreads();
-      for (int e = tid; e < F1 * kGC; e += 256) {
-        int f = e / kGC, i = e % kGC, n = n0 + i;
-        At[f * kGC + i] = (n < N) ? (f < F ? al[(long)f * Npad + n] : ga[n]) : T(0);
+      for (int e = tid; e < nf * kGC; e += 256) {
+        int f = f0 + e / kGC, i = e % kGC, n = n0 + i;
+        At[e] = (n < N) ? (f < F ? al[(long)f * Npad + n] : ga[n]) : T(0);
       }
       __syncthreads();
 #pragma unroll
       for (int r = 0; r < R; ++r) {
         int p = p0 + r * 256 + tid;
-        if (p < npairs) {
-          int f = p / D1, d = p % D1;
+        if (p < p1) {
+          int f = p / D1 - f0, d = p % D1;
           T a = acc[r];
           for (int i = 0; i < kGC; ++i) a = fma(At[f * kGC + i], Tt[i * D1 + d], a);
           acc[r] = a;
@@ -105,7 +114,7 @@ __global__ void __launch_bounds__(256) ei_grad_terms_kernel(int kind, int N, int
 #pragma unroll
     for (int r = 0; r < R; ++r) {
       int p = p0 + r * 256 + tid;
-      if (p < npairs) o[p] = acc[r];
+      if (p < p1) o[p] = acc[r];
     }
   }
 }
@@ -120,7 +129,8 @@ int ei_grad_terms(int kind, int N, int Npad, int D, int S, int Q, int F, const T
   if (Q <= 0) return -6;
   if (F <= 0) return -7;
   if (!X || !xq || !inv_ls || !amp2 || !alpha || !gamma || !out) return -8;
-  const size_t dsm = sizeof(T) * ((size_t)kGC * (D + 1) + (size_t)(F + 1) * kGC + 2 * (size_t)D);
+  // F adds at most kFR rows; D alone can exceed the budget (D > 324 in float64, D > 712 in float32)
+  const size_t dsm = sizeof(T) * ((size_t)kGC * (D + 1) + (size_t)ei_grad_rows(F) * kGC + 2 * (size_t)D);
   if (dsm > 200 * 1024) return -4;
   static size_t attr_set = 48 * 1024;
   if (dsm > attr_set) {
