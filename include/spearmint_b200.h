@@ -272,6 +272,28 @@ int smk_ei_sweep_weighted_f32(int M, int S, int F, const float* mu, const float*
 int smk_ei_sweep_weighted_f64(int M, int S, int F, const double* mu, const double* var, int ldm, const double* best,
                               const double* w, double* ei, double* ei_sum, unsigned long long* ei_max, void* stream);
 
+/* ---- (5c) random forest (RF = chooser/RandomForestEIChooser.py)
+ * smk_forest_fit_f64: grows T regression trees as scikit-learn 1.9's RandomForestRegressor does (RF:64, 72):
+ *   DepthFirstTreeBuilder + BestSplitter + MSE, min_samples_leaf 1, min_weight_leaf 0, on X [N][D] (float32, the
+ *   conversion sklearn applies), y [N], bootstrap counts w [T][N] as sample weights and the splitter's rand_r state per
+ *   tree, rand_r_state [T] -- both drawn on the host from numpy's RNG.  max_depth: INT32_MAX for none;
+ *   min_samples_split >= 2.  Node arrays [T][ldn], ldn >= 2N-1, in sklearn's layout and node order: feature (-2 at a
+ *   leaf), threshold (-2.0 at a leaf), left / right (-1 at a leaf), n_node_samples, value (sum_total / weighted n);
+ *   node_count [T].  One CTA per tree; D is bounded by the per-tree feature arrays in shared memory (32 D bytes, -2
+ *   beyond the opt-in limit).  workspace: smk_forest_workspace_bytes(N, D, T).
+ * smk_forest_predict_ei_f64: for each candidate C [M][D] (float32), mean = (sum of the T leaf values in tree order)/T,
+ *   var = sum_t (leaf_t - mean)^2 / (T-1) (NaN for T = 1, as np.var(ddof=1)), and
+ *   ei = s (u Phi(u) + phi(u)), s = sqrt(var) + 1e-4, u = (best - mean)/s  (RF:16-26, 80-85).  mean, var and ei are
+ *   optional outputs [M] (NULL: not written).                                                                       */
+size_t smk_forest_workspace_bytes(int N, int D, int T);
+int smk_forest_fit_f64(int N, int D, int T, const float* X, const double* y, const double* w,
+                       const uint32_t* rand_r_state, int max_features, int max_depth, int min_samples_split, int ldn,
+                       int* feature, double* threshold, int* left, int* right, int* n_node_samples, double* value,
+                       int* node_count, void* workspace, size_t workspace_bytes, void* stream);
+int smk_forest_predict_ei_f64(int M, int D, int T, int ldn, const float* C, const int* feature, const double* threshold,
+                              const int* left, const int* right, const double* value, double best, double* mean,
+                              double* var, double* ei, void* stream);
+
 /* ---- (6) selection: argsort(mean)[-k:] and argmax(mean)   (OPT:270-271, OPT:294)
  * score: [M].  idx_out[k]: indices of the k largest scores in ASCENDING score order (so
  * idx_out[k-1] is the argmax; ties resolved towards the lower index, numpy's first-max rule).

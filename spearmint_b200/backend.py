@@ -8,6 +8,10 @@
     refine_context(...)                           -> object with value_grad(x)                   (f1, OPT:360-525)
     constrained_ei_matrix(kind, hs, constraint_hs, ff, comp, labels, pend, cand, vals, normals)
                                                   -> (M, S) float64 numpy, constrained EI        (CONS:450-468)
+    forest_fit(X, y, weights, rand_r_states, max_features, max_depth, min_samples_split)
+                                                  -> forest grown on the GPU                     (RF:64, 72)
+    forest_predict(forest, X)                     -> (mean, var) float64 numpy                   (RF:16-26)
+    forest_argmax_ei(forest, cand, best)          -> index of the largest RF EI                  (RF:75-87)
 
 The chooser classes only talk to this interface, so the host logic (RNG order, state files, return protocol)
 can be unit-tested on a CPU-only box with a stand-in backend supplied by the test; the product always constructs
@@ -202,6 +206,27 @@ class DeviceBackend(object):
         """object with value_grad(x): CONS:471-803 summed over the sample pairs, factors cached."""
         return self.refine_eng.constrained_refine_context(kind, hyper_samples, chyper_samples, ff, comp, labels, pend,
                                                           vals, normals, noise)
+
+    # ---- random forest (RF = chooser/RandomForestEIChooser.py); every rank grows the same forest
+    def forest_fit(self, X, y, weights, rand_r_states, max_features, max_depth=None, min_samples_split=2):
+        """T regression trees grown on the GPU from the host draws of forest.draws (RF:64, 72)."""
+        from .forest import DeviceForest
+        eng = self.eng64
+        return DeviceForest(eng.device, eng.stream(), X, y, weights, rand_r_states, max_features, max_depth,
+                            min_samples_split)
+
+    def forest_predict(self, forest, X):
+        """(mean, var) float64 numpy at X (RF:16-26)."""
+        out = forest.predict(X, want=("mean", "var"))
+        return out["mean"].cpu().numpy(), out["var"].cpu().numpy()
+
+    def forest_argmax_ei(self, forest, cand, best):
+        """argmax of the RF EI (RF:80-87) over the candidates, numpy's first-max rule: the device top-k."""
+        M = cand.shape[0]
+        ei = forest.predict(cand, best, want=("ei",))["ei"]
+        idx, _ = self.eng64.topk(ei, M, 1)
+        i = int(idx[0].item())
+        return 0 if i < 0 else i         # every EI NaN (a single tree: var is NaN): np.argmax returns 0
 
     # ---- f1
     def refine_context(self, kind, hyper_samples, comp, pend, vals, normals=None, time_hyper_samples=None,

@@ -111,6 +111,11 @@ size_t tc_guard_workspace_bytes(int, int);
 int tc_guard(int, int, int, int, const float*, const float*, const float*, const float*, const float*, const int*, float*, void*,
              size_t, cudaStream_t);
 int potrf_ll_f64(int, int, double*, double*, int*, int, cudaStream_t);
+size_t forest_workspace_bytes(int, int, int);
+int forest_fit(int, int, int, const float*, const double*, const double*, const uint32_t*, int, int, int, int, int*,
+               double*, int*, int*, int*, double*, int*, void*, size_t, cudaStream_t);
+int forest_predict_ei(int, int, int, int, const float*, const int*, const double*, const int*, const int*, const double*,
+                      double, double*, double*, double*, cudaStream_t);
 
 }  // namespace smk
 
@@ -349,6 +354,20 @@ int smk_constraint_prob_f64(int kind, int N, int Npad, int M, int D, int S, cons
                             double* p_out, double* m_out, int ldm, void* stream) {
   return constraint_prob<double>(kind, N, Npad, M, D, S, X, C, inv_ls, amp2, t_alpha, gain, p_out, m_out, ldm,
                                  ST(stream));
+}
+
+size_t smk_forest_workspace_bytes(int N, int D, int T) { return forest_workspace_bytes(N, D, T); }
+int smk_forest_fit_f64(int N, int D, int T, const float* X, const double* y, const double* w,
+                       const uint32_t* rand_r_state, int max_features, int max_depth, int min_samples_split, int ldn,
+                       int* feature, double* threshold, int* left, int* right, int* n_node_samples, double* value,
+                       int* node_count, void* workspace, size_t workspace_bytes, void* stream) {
+  return forest_fit(N, D, T, X, y, w, rand_r_state, max_features, max_depth, min_samples_split, ldn, feature, threshold,
+                    left, right, n_node_samples, value, node_count, workspace, workspace_bytes, ST(stream));
+}
+int smk_forest_predict_ei_f64(int M, int D, int T, int ldn, const float* C, const int* feature, const double* threshold,
+                              const int* left, const int* right, const double* value, double best, double* mean,
+                              double* var, double* ei, void* stream) {
+  return forest_predict_ei(M, D, T, ldn, C, feature, threshold, left, right, value, best, mean, var, ei, ST(stream));
 }
 
 size_t smk_topk_workspace_bytes(int M, int k) { return topk_workspace_bytes(M, k); }
