@@ -22,9 +22,6 @@ sums over fantasies; the second grid pass scores the refined AND the unrefined s
 whose result the reference never uses are skipped.  Extra optional keys: ``device``, ``refine_dtype``, ``state_name``.
 """
 import math
-import os
-import pickle
-import tempfile
 
 import numpy as np
 import numpy.random as npr
@@ -32,9 +29,8 @@ import scipy.optimize as spo
 import scipy.stats as sps
 
 from spearmint_b200 import util
-from spearmint_b200.locker import Locker, log
-
-COVARS = ("SE", "ARDSE", "Matern32", "Matern52")
+from spearmint_b200.chooser._gp import GPChooser, GPPrior, write_state, write_stats
+from spearmint_b200.locker import log
 
 
 def init(expt_dir, arg_string):
@@ -73,86 +69,45 @@ def elliptical_slice(xx, factor, log_like_fn):
         phi = npr.rand() * (phi_max - phi_min) + phi_min
 
 
-class GPConstrainedEIChooserB200(object):
+class GPConstrainedEIChooserB200(GPChooser):
+    prior = GPPrior(max_ls=2, noise_times_amp2=True)      # K = amp2 (k + 1e-6 I + noise I) in the joint move only
 
     def __init__(self, expt_dir, covar="Matern52", mcmc_iters=20, pending_samples=100, noiseless=False, burnin=100,
                  grid_subset=20, constraint_violating_value=np.inf, verbosity=0, visualize2D=False, device=None,
                  refine_dtype="float64", state_name=None, backend=None):
-        if covar not in COVARS:
-            raise AttributeError("module 'spearmint.gp' has no attribute '%s'" % covar)   # getattr(gp, covar), CONS:67
+        GPChooser.__init__(self, expt_dir, covar, mcmc_iters, pending_samples, noiseless, state_name, device, backend,
+                           refine_dtype)
         if visualize2D:      # an arg string hands over a non-empty str, which the reference treats as true (CONS:308)
             raise NotImplementedError("visualize2D: the 2-D contour plots of the reference are not provided")
-        self.covar = covar
-        self.locker = Locker()
-        name = state_name if state_name else self.__module__
-        self.state_pkl = os.path.join(expt_dir, name + ".pkl")
-        self.stats_file = os.path.join(expt_dir, name + "_hyperparameters.txt")
-        self.mcmc_iters = int(mcmc_iters)
         self.burnin = int(burnin)
         self.needs_burnin = True
-        self.pending_samples = int(pending_samples)
-        self.D = -1
-        self.hyper_iters = 1
         self.grid_subset = int(grid_subset)
-        self.noiseless = bool(int(noiseless))
         self.hyper_samples = []
         self.constraint_hyper_samples = []
         self.ff = None
         self.ff_samples = []
         self.verbosity = int(verbosity)
-        self.noise_scale = 0.1            # horseshoe prior
-        self.amp2_scale = 1               # zero-mean log normal prior
-        self.max_ls = 2                   # top-hat prior on length scales
         self.constraint_noise_scale = 0.1
         self.constraint_amp2_scale = 1
         self.constraint_gain = 1
         self.constraint_max_ls = 2
         self.bad_value = float(constraint_violating_value)
         self.visualize2D = visualize2D
-        self._device, self._refine_dtype = device, refine_dtype
-        self._backend = backend
-
-    @property
-    def backend(self):
-        if self._backend is None:
-            from spearmint_b200.backend import DeviceBackend
-            self._backend = DeviceBackend(device=self._device, refine_dtype=self._refine_dtype)
-        return self._backend
 
     # ------------------------------------------------------------------ state files (CONS:101-191)
     def dump_hypers(self):
-        self.locker.lock_wait(self.state_pkl)
-        fh = tempfile.NamedTemporaryFile(mode="wb", delete=False)
-        pickle.dump({"dims": self.D, "ls": self.ls, "amp2": self.amp2, "noise": self.noise, "mean": self.mean,
+        write_state(self.locker, self.state_pkl,
+                    {"dims": self.D, "ls": self.ls, "amp2": self.amp2, "noise": self.noise, "mean": self.mean,
                      "constraint_ls": self.constraint_ls, "constraint_amp2": self.constraint_amp2,
                      "constraint_noise": self.constraint_noise, "constraint_mean": self.constraint_mean,
-                     "constraint_gain": self.constraint_gain}, fh, protocol=2)
-        fh.close()
-        os.system('mv "%s" "%s"' % (fh.name, self.state_pkl))       # atomic move, as the reference
-        self.locker.unlock(self.state_pkl)
-
-        with open(self.stats_file, "w") as fh:
-            fh.write("Mean Noise Amplitude <length scales>\n")
-            fh.write("-----------ALL SAMPLES-------------\n")
-            meanhyps = 0 * np.hstack(self.hyper_samples[0])
-            for h in self.hyper_samples:
-                hyps = np.hstack(h)
-                meanhyps += (1 / float(len(self.hyper_samples))) * hyps
-                fh.write(" ".join(str(j) for j in hyps) + " \n")
-            fh.write("-----------MEAN OF SAMPLES-------------\n")
-            fh.write(" ".join(str(j) for j in meanhyps) + " \n")
+                     "constraint_gain": self.constraint_gain})
+        write_stats(self.stats_file, self.hyper_samples)
 
     def _real_init(self, dims, values):
-        self.locker.lock_wait(self.state_pkl)
         self.randomstate = npr.get_state()
-        if os.path.exists(self.state_pkl):
-            with open(self.state_pkl, "rb") as fh:
-                state = pickle.load(fh)
-            self.D = state["dims"]
-            self.ls = state["ls"]
-            self.amp2 = state["amp2"]
-            self.noise = state["noise"]
-            self.mean = state["mean"]
+        state = self._read_state()
+        if state is not None:
+            self._load_hypers(state)
             self.constraint_ls = state["constraint_ls"]
             self.constraint_amp2 = state["constraint_amp2"]
             self.constraint_noise = state["constraint_noise"]
@@ -161,17 +116,12 @@ class GPConstrainedEIChooserB200(object):
             self.needs_burnin = False
         else:
             goodvals = np.nonzero(np.logical_and(values != self.bad_value, np.isfinite(values)))[0]
-            self.D = dims
-            self.ls = np.ones(self.D)
+            self._init_hypers(dims, values[goodvals])
             self.constraint_ls = np.ones(self.D)
-            self.amp2 = np.std(values[goodvals]) + 1e-4
             self.constraint_amp2 = 1.0
-            self.noise = 1e-3
             self.constraint_noise = 1e-3
             self.constraint_gain = 1
-            self.mean = np.mean(values[goodvals])
             self.constraint_mean = 0.5
-        self.locker.unlock(self.state_pkl)
 
     # ------------------------------------------------------------------ the plugin entry point (CONS:203-422)
     def next(self, grid, values, durations, candidates, pending, complete):
@@ -365,59 +315,11 @@ class GPConstrainedEIChooserB200(object):
 
     # ------------------------------------------------------------------ objective chain (CONS:1032-1056, 1116-1232)
     def sample_hypers(self, comp, vals):
+        """CONS:1116-1149: the joint move scales the noise by amp2, the length-scale move does not (CONS:1047-1049)."""
+        ll = self._ll(comp, vals)
         if self.noiseless:
             self.noise = 1e-3
-            self._sample_noiseless(comp, vals)
-        else:
-            self._sample_noisy(comp, vals)
-        self._sample_ls(comp, vals)
+        self.mean, self.amp2, self.noise = self.prior.joint(ll, self.mean, self.amp2, self.noise, self.ls, vals,
+                                                            self.noiseless)
+        self.ls = self.prior.length_scales(ll, self.mean, self.noise, self.amp2, self.ls)
         self.hyper_samples.append((self.mean, self.noise, self.amp2, self.ls))
-
-    def _ll(self, comp, vals):
-        if getattr(self, "_loglik", None) is None:
-            self._loglik = self.backend.loglik(self.covar, comp, vals)
-        return self._loglik
-
-    def _sample_ls(self, comp, vals):
-        mean, noise, amp2, max_ls = self.mean, self.noise, self.amp2, self.max_ls
-
-        def hypers_of(ls):
-            if np.any(ls < 0) or np.any(ls > max_ls):
-                return None
-            return (mean, noise, amp2, ls), ()
-
-        self.ls = util.slice_sample(self.ls, util.make_logprob(self._ll(comp, vals), hypers_of), compwise=True)
-
-    def _sample_noisy(self, comp, vals):
-        """CONS:1116-1149: here the noise is scaled by amp2 as well, K = amp2 (k + 1e-6 I + noise I), and the amplitude
-        prior is on log(amp2) (GPEIOptChooser: on log(sqrt(amp2)))."""
-        vmax, vmin, ls = np.max(vals), np.min(vals), self.ls
-
-        def hypers_of(hypers):
-            mean, amp2, noise = hypers[0], hypers[1], hypers[2]
-            if mean > vmax or mean < vmin:
-                return None
-            if amp2 < 0 or noise < 0:
-                return None
-            return (mean, amp2 * noise, amp2, ls), (
-                np.log(np.log(1 + (self.noise_scale / noise) ** 2)),
-                -0.5 * (np.log(amp2) / self.amp2_scale) ** 2)
-
-        hypers = util.slice_sample(np.array([self.mean, self.amp2, self.noise]),
-                                   util.make_logprob(self._ll(comp, vals), hypers_of), compwise=False)
-        self.mean, self.amp2, self.noise = hypers[0], hypers[1], hypers[2]
-
-    def _sample_noiseless(self, comp, vals):
-        vmax, vmin, ls = np.max(vals), np.min(vals), self.ls
-
-        def hypers_of(hypers):
-            mean, amp2 = hypers[0], hypers[1]
-            if mean > vmax or mean < vmin:
-                return None
-            if amp2 < 0:
-                return None
-            return (mean, amp2 * 1e-3, amp2, ls), (-0.5 * (np.log(amp2) / self.amp2_scale) ** 2,)
-
-        hypers = util.slice_sample(np.array([self.mean, self.amp2, self.noise]),
-                                   util.make_logprob(self._ll(comp, vals), hypers_of), compwise=False)
-        self.mean, self.amp2, self.noise = hypers[0], hypers[1], 1e-3

@@ -8,17 +8,12 @@ done for all samples in ONE batched GPU pass (``compute_ei`` math is identical t
 State pickle keys dims/ls/amp2/noise/mean, written on destruction like the reference (GPEI:66-84).
 ``mcmc_iters=0`` runs the ML-II branch: ``gp.GP.optimize_hypers`` (spearmint_b200/gp.py, GP:181-292) then EI under the optimum.
 """
-import os
-import pickle
-import tempfile
-
 import numpy as np
 import numpy.random as npr
 
 from spearmint_b200 import util
-from spearmint_b200.locker import Locker, log
-
-COVARS = ("SE", "ARDSE", "Matern32", "Matern52")
+from spearmint_b200.chooser._gp import GPChooser, GPPrior, write_state
+from spearmint_b200.locker import log
 
 
 def init(expt_dir, arg_string):
@@ -26,42 +21,18 @@ def init(expt_dir, arg_string):
     return GPEIChooserB200(expt_dir, **args)
 
 
-class GPEIChooserB200(object):
+class GPEIChooserB200(GPChooser):
+    prior = GPPrior(max_ls=2)
 
     def __init__(self, expt_dir, covar="Matern52", mcmc_iters=10, pending_samples=100, noiseless=False,
                  device=None, state_name=None, backend=None):
-        if covar not in COVARS:
-            raise AttributeError("module 'spearmint.gp' has no attribute '%s'" % covar)
-        self.covar = covar
-        self.locker = Locker()
-        name = state_name if state_name else self.__module__
-        self.state_pkl = os.path.join(expt_dir, name + ".pkl")
-        self.mcmc_iters = int(mcmc_iters)
-        self.pending_samples = int(pending_samples)
-        self.D = -1
-        self.hyper_iters = 1
-        self.noiseless = bool(int(noiseless))
-        self.noise_scale, self.amp2_scale, self.max_ls = 0.1, 1, 2
-        self._device, self._backend = device, backend
-        self._ll = None
-
-    @property
-    def backend(self):
-        if self._backend is None:
-            from spearmint_b200.backend import DeviceBackend
-            self._backend = DeviceBackend(device=self._device)
-        return self._backend
+        GPChooser.__init__(self, expt_dir, covar, mcmc_iters, pending_samples, noiseless, state_name, device, backend)
 
     def dump_hypers(self):
         if self.D == -1:
             return
-        self.locker.lock_wait(self.state_pkl)
-        fh = tempfile.NamedTemporaryFile(mode="wb", delete=False)
-        pickle.dump({"dims": self.D, "ls": self.ls, "amp2": self.amp2, "noise": self.noise, "mean": self.mean},
-                    fh, protocol=2)
-        fh.close()
-        os.system('mv "%s" "%s"' % (fh.name, self.state_pkl))
-        self.locker.unlock(self.state_pkl)
+        write_state(self.locker, self.state_pkl,
+                    {"dims": self.D, "ls": self.ls, "amp2": self.amp2, "noise": self.noise, "mean": self.mean})
 
     def __del__(self):          # the reference persists its state in the destructor (GPEI:66-84)
         try:
@@ -70,19 +41,11 @@ class GPEIChooserB200(object):
             pass
 
     def _real_init(self, dims, values):
-        self.locker.lock_wait(self.state_pkl)
-        if os.path.exists(self.state_pkl):
-            with open(self.state_pkl, "rb") as fh:
-                state = pickle.load(fh)
-            self.D, self.ls, self.amp2 = state["dims"], state["ls"], state["amp2"]
-            self.noise, self.mean = state["noise"], state["mean"]
+        state = self._read_state()
+        if state is not None:
+            self._load_hypers(state)
         else:
-            self.D = dims
-            self.ls = np.ones(self.D)
-            self.amp2 = np.std(values) + 1e-4
-            self.noise = 1e-3
-            self.mean = np.mean(values)
-        self.locker.unlock(self.state_pkl)
+            self._init_hypers(dims, values)
 
     def next(self, grid, values, durations, candidates, pending, complete):
         if complete.shape[0] < 2:
@@ -104,7 +67,7 @@ class GPEIChooserB200(object):
             ei = self.compute_ei(comp, pend, cand, vals)
             return int(candidates[int(np.argmax(ei))])
         P = pend.shape[0]
-        self._ll = self.backend.loglik(self.covar, comp, vals)
+        self._loglik = self.backend.loglik(self.covar, comp, vals)
         hs, normals = [], []
         for mcmc_iter in range(self.mcmc_iters):
             self.sample_hypers(comp, vals)
@@ -113,7 +76,7 @@ class GPEIChooserB200(object):
             hs.append((self.mean, self.noise, self.amp2, self.ls))
             if P:
                 normals.append(npr.randn(P, self.pending_samples))       # same stream position as GPEI:237
-        self._ll = None
+        self._loglik = None
         st = self.backend.grid_state(self.covar, hs, comp, pend, vals, np.array(normals) if P else None)
         best_cand = int(self.backend.top_mean_ei(st, cand, 1)[-1])
         return int(candidates[best_cand])
@@ -132,50 +95,9 @@ class GPEIChooserB200(object):
 
     # ------------------------------------------------------------------ sampling (GPEI:268-346)
     def sample_hypers(self, comp, vals):
-        if self._ll is None:
-            self._ll = self.backend.loglik(self.covar, comp, vals)
+        ll = self._ll(comp, vals)
         if self.noiseless:
             self.noise = 1e-3
-            self._sample_noiseless(comp, vals)
-        else:
-            self._sample_noisy(comp, vals)
-        self._sample_ls(comp, vals)
-
-    def _sample_ls(self, comp, vals):
-        mean, noise, amp2, max_ls = self.mean, self.noise, self.amp2, self.max_ls
-
-        def hypers_of(ls):
-            if np.any(ls < 0) or np.any(ls > max_ls):
-                return None
-            return (mean, noise, amp2, ls), ()
-        self.ls = util.slice_sample(self.ls, util.make_logprob(self._ll, hypers_of), compwise=True)
-
-    def _sample_noisy(self, comp, vals):
-        vmax, vmin, ls = np.max(vals), np.min(vals), self.ls
-
-        def hypers_of(hypers):
-            mean, amp2, noise = hypers[0], hypers[1], hypers[2]
-            if mean > vmax or mean < vmin:
-                return None
-            if amp2 < 0 or noise < 0:
-                return None
-            return (mean, noise, amp2, ls), (
-                np.log(np.log(1 + (self.noise_scale / noise) ** 2)),
-                -0.5 * (np.log(amp2) / self.amp2_scale) ** 2)              # log(amp2): GPEI:312
-        hypers = util.slice_sample(np.array([self.mean, self.amp2, self.noise]),
-                                   util.make_logprob(self._ll, hypers_of), compwise=False)
-        self.mean, self.amp2, self.noise = hypers[0], hypers[1], hypers[2]
-
-    def _sample_noiseless(self, comp, vals):
-        vmax, vmin, ls = np.max(vals), np.min(vals), self.ls
-
-        def hypers_of(hypers):
-            mean, amp2 = hypers[0], hypers[1]
-            if mean > vmax or mean < vmin:
-                return None
-            if amp2 < 0:
-                return None
-            return (mean, 1e-3, amp2, ls), (-0.5 * (np.log(amp2) / self.amp2_scale) ** 2,)
-        hypers = util.slice_sample(np.array([self.mean, self.amp2, self.noise]),
-                                   util.make_logprob(self._ll, hypers_of), compwise=False)
-        self.mean, self.amp2, self.noise = hypers[0], hypers[1], 1e-3
+        self.mean, self.amp2, self.noise = self.prior.joint(ll, self.mean, self.amp2, self.noise, self.ls, vals,
+                                                            self.noiseless)
+        self.ls = self.prior.length_scales(ll, self.mean, self.noise, self.amp2, self.ls)

@@ -15,9 +15,6 @@ evaluation is a hand-written sm_90a kernel behind the C ABI (``spearmint_b200.ba
 ``use_multiprocessing`` is accepted and ignored: a forked pool cannot share a CUDA context, and with cached
 factors the 20 refinements are cheap.  Extra optional keys: ``device``, ``refine_dtype``, ``state_name``.
 """
-import os
-import pickle
-import tempfile
 import time
 
 import numpy as np
@@ -25,9 +22,8 @@ import numpy.random as npr
 import scipy.optimize as spo
 
 from spearmint_b200 import util
-from spearmint_b200.locker import Locker, log
-
-COVARS = ("SE", "ARDSE", "Matern32", "Matern52")     # the stationary kernels of gp.py:87-127
+from spearmint_b200.chooser._gp import GPChooser, GPPrior, read_state, write_state, write_stats
+from spearmint_b200.locker import log
 
 
 def init(expt_dir, arg_string):
@@ -35,84 +31,37 @@ def init(expt_dir, arg_string):
     return GPEIOptChooserB200(expt_dir, **args)
 
 
-class GPEIOptChooserB200(object):
+class GPEIOptChooserB200(GPChooser):
+    prior = GPPrior(max_ls=2, amp2_prior_on_std=True)
 
     def __init__(self, expt_dir, covar="Matern52", mcmc_iters=10, pending_samples=100, noiseless=False, burnin=100,
                  grid_subset=20, use_multiprocessing=True, device=None, refine_dtype="float64", state_name=None,
                  backend=None):
-        if covar not in COVARS:
-            raise AttributeError("module 'spearmint.gp' has no attribute '%s'" % covar)   # getattr(gp, covar), OPT:57
-        self.covar = covar
-        self.locker = Locker()
-        name = state_name if state_name else self.__module__
-        self.state_pkl = os.path.join(expt_dir, name + ".pkl")
-        self.stats_file = os.path.join(expt_dir, name + "_hyperparameters.txt")
-        self.mcmc_iters = int(mcmc_iters)
+        GPChooser.__init__(self, expt_dir, covar, mcmc_iters, pending_samples, noiseless, state_name, device, backend,
+                           refine_dtype)
         self.burnin = int(burnin)
         self.needs_burnin = True
-        self.pending_samples = int(pending_samples)
-        self.D = -1
-        self.hyper_iters = 1
         self.grid_subset = int(grid_subset)
-        self.noiseless = bool(int(noiseless))
         self.hyper_samples = []
-        self.noise_scale = 0.1     # horseshoe prior
-        self.amp2_scale = 1        # zero-mean log normal prior
-        self.max_ls = 2            # top-hat prior on length scales
         self.use_multiprocessing = bool(int(use_multiprocessing))
-        self._device, self._refine_dtype = device, refine_dtype
-        self._backend = backend
         self.stats = {}
-
-    # ------------------------------------------------------------------ backend (GPU; raises if unavailable)
-    @property
-    def backend(self):
-        if self._backend is None:
-            from spearmint_b200.backend import DeviceBackend
-            self._backend = DeviceBackend(device=self._device, refine_dtype=self._refine_dtype)
-        return self._backend
 
     # ------------------------------------------------------------------ state files (OPT:84-120, 150-205)
     def dump_hypers(self):
-        self.locker.lock_wait(self.state_pkl)
-        fh = tempfile.NamedTemporaryFile(mode="wb", delete=False)
-        pickle.dump({"dims": self.D, "ls": self.ls, "amp2": self.amp2, "noise": self.noise,
-                     "hyper_samples": self.hyper_samples, "mean": self.mean}, fh, protocol=2)
-        fh.close()
-        os.system('mv "%s" "%s"' % (fh.name, self.state_pkl))       # atomic move, as the reference
-        self.locker.unlock(self.state_pkl)
+        write_state(self.locker, self.state_pkl, {"dims": self.D, "ls": self.ls, "amp2": self.amp2, "noise": self.noise,
+                                                  "hyper_samples": self.hyper_samples, "mean": self.mean})
+        write_stats(self.stats_file, self.hyper_samples)
 
-        with open(self.stats_file, "w") as fh:
-            fh.write("Mean Noise Amplitude <length scales>\n")
-            fh.write("-----------ALL SAMPLES-------------\n")
-            meanhyps = 0 * np.hstack(self.hyper_samples[0])
-            for h in self.hyper_samples:
-                hyps = np.hstack(h)
-                meanhyps += (1 / float(len(self.hyper_samples))) * hyps
-                fh.write(" ".join(str(j) for j in hyps) + " \n")
-            fh.write("-----------MEAN OF SAMPLES-------------\n")
-            fh.write(" ".join(str(j) for j in meanhyps) + " \n")
-
-    def _load_state(self):
-        with open(self.state_pkl, "rb") as fh:
-            state = pickle.load(fh)
-        self.D = state["dims"]
-        self.ls = state["ls"]
-        self.amp2 = state["amp2"]
-        self.noise = state["noise"]
-        self.mean = state["mean"]
+    def _load_state(self, state):
+        self._load_hypers(state)
         self.hyper_samples = state["hyper_samples"]
         self.needs_burnin = False
 
-    def _read_only(self):
-        if os.path.exists(self.state_pkl):
-            self._load_state()
-            return True
-        return False
-
     def generate_stats_html(self):
-        if not self._read_only():
+        state = read_state(self.state_pkl)
+        if state is None:
             return "Chooser not yet ready to display output"
+        self._load_state(state)
         mean_mean = np.mean(np.vstack([h[0] for h in self.hyper_samples]))
         mean_noise = np.mean(np.vstack([h[1] for h in self.hyper_samples]))
         mean_ls = np.mean(np.vstack([h[3][np.newaxis, :] for h in self.hyper_samples]), 0)
@@ -125,22 +74,17 @@ class GPEIOptChooserB200(object):
                       'var lsdata = [' + ','.join(['%.2f' % i for i in mean_ls]) + '];')
         except Exception:
             return "Chooser not yet ready to display output."
-        output += 'bar_chart("#lschart", lsdata, ' + str(self.max_ls) + ');' + '</script>'
+        output += 'bar_chart("#lschart", lsdata, ' + str(self.prior.max_ls) + ');' + '</script>'
         return output
 
     def _real_init(self, dims, values):
-        self.locker.lock_wait(self.state_pkl)
         self.randomstate = npr.get_state()
-        if os.path.exists(self.state_pkl):
-            self._load_state()
+        state = self._read_state()
+        if state is not None:
+            self._load_state(state)
         else:
-            self.D = dims
-            self.ls = np.ones(self.D)
-            self.amp2 = np.std(values) + 1e-4       # a std, not a variance -- reference quirk kept (OPT:193)
-            self.noise = 1e-3
-            self.mean = np.mean(values)
+            self._init_hypers(dims, values)
             self.hyper_samples.append((self.mean, self.noise, self.amp2, self.ls))
-        self.locker.unlock(self.state_pkl)
 
     # ------------------------------------------------------------------ the plugin entry point (OPT:217-328)
     def next(self, grid, values, durations, candidates, pending, complete):
@@ -261,58 +205,11 @@ class GPEIOptChooserB200(object):
         return (f, g) if compute_grad else f
 
     # ------------------------------------------------------------------ hyper-parameter sampling (OPT:621-706)
-    def _ll(self, comp, vals):
-        if getattr(self, "_loglik", None) is None:
-            self._loglik = self.backend.loglik(self.covar, comp, vals)
-        return self._loglik
-
     def sample_hypers(self, comp, vals):
+        ll = self._ll(comp, vals)
         if self.noiseless:
             self.noise = 1e-3
-            self._sample_noiseless(comp, vals)
-        else:
-            self._sample_noisy(comp, vals)
-        self._sample_ls(comp, vals)
+        self.mean, self.amp2, self.noise = self.prior.joint(ll, self.mean, self.amp2, self.noise, self.ls, vals,
+                                                            self.noiseless)
+        self.ls = self.prior.length_scales(ll, self.mean, self.noise, self.amp2, self.ls)
         self.hyper_samples.append((self.mean, self.noise, self.amp2, self.ls))
-
-    def _sample_ls(self, comp, vals):
-        mean, noise, amp2, max_ls = self.mean, self.noise, self.amp2, self.max_ls
-
-        def hypers_of(ls):
-            if np.any(ls < 0) or np.any(ls > max_ls):
-                return None
-            return (mean, noise, amp2, ls), ()
-
-        self.ls = util.slice_sample(self.ls, util.make_logprob(self._ll(comp, vals), hypers_of), compwise=True)
-
-    def _sample_noisy(self, comp, vals):
-        vmax, vmin, ls = np.max(vals), np.min(vals), self.ls
-
-        def hypers_of(hypers):
-            mean, amp2, noise = hypers[0], hypers[1], hypers[2]
-            if mean > vmax or mean < vmin:
-                return None
-            if amp2 < 0 or noise < 0:
-                return None
-            return (mean, noise, amp2, ls), (
-                np.log(np.log(1 + (self.noise_scale / noise) ** 2)),           # horseshoe prior on the noise
-                -0.5 * (np.log(np.sqrt(amp2)) / self.amp2_scale) ** 2)        # log-normal prior on the amplitude
-
-        hypers = util.slice_sample(np.array([self.mean, self.amp2, self.noise]),
-                                   util.make_logprob(self._ll(comp, vals), hypers_of), compwise=False)
-        self.mean, self.amp2, self.noise = hypers[0], hypers[1], hypers[2]
-
-    def _sample_noiseless(self, comp, vals):
-        vmax, vmin, ls = np.max(vals), np.min(vals), self.ls
-
-        def hypers_of(hypers):
-            mean, amp2 = hypers[0], hypers[1]
-            if mean > vmax or mean < vmin:
-                return None
-            if amp2 < 0:
-                return None
-            return (mean, 1e-3, amp2, ls), (-0.5 * (np.log(np.sqrt(amp2)) / self.amp2_scale) ** 2,)
-
-        hypers = util.slice_sample(np.array([self.mean, self.amp2, self.noise]),
-                                   util.make_logprob(self._ll(comp, vals), hypers_of), compwise=False)
-        self.mean, self.amp2, self.noise = hypers[0], hypers[1], 1e-3

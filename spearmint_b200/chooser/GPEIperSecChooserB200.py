@@ -7,21 +7,16 @@ because they decide which point it proposes (SURVEY.md 3.4 / section 7):
   * ``time_hyper_samples`` is never cleared (PSEC:199), so index [i] reads the OLDEST (burn-in) time samples (PSEC:288);
   * the refinement ignores pending points (PSEC:351-435) and is serial;
   * fantasy normals come straight from the global RNG stream, with no state reset (PSEC:521);
-  * max_ls = 10; objective amp2 prior log(amp2) (PSEC:614), time-GP amp2 prior log(sqrt(amp2)) (PSEC:646).
+  * the objective and time chains are sampled with GPPrior values of their own (chooser/_gp.py).
 All arithmetic runs on the GPU through spearmint_b200.backend.DeviceBackend.
 """
-import os
-import pickle
-import tempfile
-
 import numpy as np
 import numpy.random as npr
 import scipy.optimize as spo
 
 from spearmint_b200 import util
-from spearmint_b200.locker import Locker, log
-
-COVARS = ("SE", "ARDSE", "Matern32", "Matern52")
+from spearmint_b200.chooser._gp import GPChooser, GPPrior, write_state
+from spearmint_b200.locker import log
 
 
 def init(expt_dir, arg_string):
@@ -29,71 +24,40 @@ def init(expt_dir, arg_string):
     return GPEIperSecChooserB200(expt_dir, **args)
 
 
-class GPEIperSecChooserB200(object):
+class GPEIperSecChooserB200(GPChooser):
+    prior = GPPrior(max_ls=10)                                   # log(amp2) prior: PSEC:614
+    time_prior = GPPrior(max_ls=10, amp2_prior_on_std=True)      # log(sqrt(amp2)) prior: PSEC:646
 
     def __init__(self, expt_dir, covar="Matern52", mcmc_iters=10, pending_samples=100, noiseless=False, burnin=100,
                  grid_subset=20, device=None, refine_dtype="float64", state_name=None, backend=None):
-        if covar not in COVARS:
-            raise AttributeError("module 'spearmint.gp' has no attribute '%s'" % covar)
-        self.covar = covar
-        self.locker = Locker()
-        name = state_name if state_name else self.__module__
-        self.state_pkl = os.path.join(expt_dir, name + ".pkl")
-        self.stats_file = os.path.join(expt_dir, name + "_hyperparameters.txt")
-        self.mcmc_iters = int(mcmc_iters)
+        GPChooser.__init__(self, expt_dir, covar, mcmc_iters, pending_samples, noiseless, state_name, device, backend,
+                           refine_dtype)
         self.burnin = int(burnin)
         self.needs_burnin = True
-        self.pending_samples = int(pending_samples)
-        self.D = -1
-        self.hyper_iters = 1
         self.grid_subset = int(grid_subset)
-        self.noiseless = bool(int(noiseless))
         self.hyper_samples = []
         self.time_hyper_samples = []
-        self.noise_scale, self.amp2_scale, self.max_ls = 0.1, 1, 10
-        self.time_noise_scale, self.time_amp2_scale, self.time_max_ls = 0.1, 1, 10
-        self._device, self._refine_dtype = device, refine_dtype
-        self._backend = backend
-        self._ll_obj = self._ll_time = None
-
-    @property
-    def backend(self):
-        if self._backend is None:
-            from spearmint_b200.backend import DeviceBackend
-            self._backend = DeviceBackend(device=self._device, refine_dtype=self._refine_dtype)
-        return self._backend
+        self._time_loglik = None
 
     # ------------------------------------------------------------------ state (PSEC:82-143)
     def dump_hypers(self):
-        self.locker.lock_wait(self.state_pkl)
-        fh = tempfile.NamedTemporaryFile(mode="wb", delete=False)
-        pickle.dump({"dims": self.D, "ls": self.ls, "amp2": self.amp2, "noise": self.noise, "mean": self.mean,
+        write_state(self.locker, self.state_pkl,
+                    {"dims": self.D, "ls": self.ls, "amp2": self.amp2, "noise": self.noise, "mean": self.mean,
                      "time_ls": self.time_ls, "time_amp2": self.time_amp2, "time_noise": self.time_noise,
-                     "time_mean": self.time_mean}, fh, protocol=2)
-        fh.close()
-        os.system('mv "%s" "%s"' % (fh.name, self.state_pkl))
-        self.locker.unlock(self.state_pkl)
+                     "time_mean": self.time_mean})
 
     def _real_init(self, dims, values, durations):
-        self.locker.lock_wait(self.state_pkl)
-        if os.path.exists(self.state_pkl):
-            with open(self.state_pkl, "rb") as fh:
-                state = pickle.load(fh)
-            self.D = state["dims"]
-            self.ls, self.amp2, self.noise, self.mean = state["ls"], state["amp2"], state["noise"], state["mean"]
+        state = self._read_state()
+        if state is not None:
+            self._load_hypers(state)
             self.time_ls, self.time_amp2 = state["time_ls"], state["time_amp2"]
             self.time_noise, self.time_mean = state["time_noise"], state["time_mean"]
         else:
-            self.D = dims
-            self.ls = np.ones(self.D)
+            self._init_hypers(dims, values)
             self.time_ls = np.ones(self.D)
-            self.amp2 = np.std(values) + 1e-4
             self.time_amp2 = np.std(durations) + 1e-4      # std of the RAW durations (PSEC:132)
-            self.noise = 1e-3
             self.time_noise = 1e-3
-            self.mean = np.mean(values)
             self.time_mean = np.mean(np.log(durations))
-        self.locker.unlock(self.state_pkl)
 
     # ------------------------------------------------------------------ plugin entry point (PSEC:155-281)
     def next(self, grid, values, durations, candidates, pending, complete):
@@ -116,8 +80,8 @@ class GPEIperSecChooserB200(object):
             raise NotImplementedError("mcmc_iters=0 is broken in the reference (GPEIperSecChooser.py:254 reads an "
                                       "undefined overall_ei) and not provided here")
 
-        self._ll_obj = self.backend.loglik(self.covar, comp, vals)
-        self._ll_time = self.backend.loglik(self.covar, comp, durs.squeeze())
+        self._loglik = self.backend.loglik(self.covar, comp, vals)
+        self._time_loglik = self.backend.loglik(self.covar, comp, durs.squeeze())
         if self.needs_burnin:
             for mcmc_iter in range(self.burnin):
                 self.sample_hypers(comp, vals, durs)
@@ -136,7 +100,7 @@ class GPEIperSecChooserB200(object):
                 % (mcmc_iter + 1, self.mcmc_iters, np.exp(self.time_mean), np.sqrt(self.time_amp2),
                    np.exp(self.time_noise), np.min(self.time_ls), np.max(self.time_ls)))
         self.dump_hypers()
-        self._ll_obj = self._ll_time = None
+        self._loglik = self._time_loglik = None
 
         # grid pass 1: only sample 0 contributes (PSEC:302) -> ranking by column 0
         k = min(self.grid_subset, cand2.shape[0])
@@ -195,80 +159,19 @@ class GPEIperSecChooserB200(object):
 
     # ------------------------------------------------------------------ sampling (PSEC:550-681)
     def sample_hypers(self, comp, vals, durs):
-        if self._ll_obj is None:
-            self._ll_obj = self.backend.loglik(self.covar, comp, vals)
-            self._ll_time = self.backend.loglik(self.covar, comp, np.asarray(durs).squeeze())
+        durs = np.asarray(durs).squeeze()
+        if self._loglik is None:
+            self._loglik = self.backend.loglik(self.covar, comp, vals)
+            self._time_loglik = self.backend.loglik(self.covar, comp, durs)
+        ll, tll = self._loglik, self._time_loglik
         if self.noiseless:
             self.noise = 1e-3
-            self._sample_noiseless(comp, vals)
-        else:
-            self._sample_noisy(comp, vals)
-        self._sample_ls(comp, vals)
-        self._sample_time_noisy(comp, np.asarray(durs).squeeze())
-        self._sample_time_ls(comp, np.asarray(durs).squeeze())
+        self.mean, self.amp2, self.noise = self.prior.joint(ll, self.mean, self.amp2, self.noise, self.ls, vals,
+                                                            self.noiseless)
+        self.ls = self.prior.length_scales(ll, self.mean, self.noise, self.amp2, self.ls)
+        # the time chain is always noisy
+        self.time_mean, self.time_amp2, self.time_noise = self.time_prior.joint(
+            tll, self.time_mean, self.time_amp2, self.time_noise, self.time_ls, durs)
+        self.time_ls = self.time_prior.length_scales(tll, self.time_mean, self.time_noise, self.time_amp2, self.time_ls)
         self.hyper_samples.append((self.mean, self.noise, self.amp2, self.ls))
         self.time_hyper_samples.append((self.time_mean, self.time_noise, self.time_amp2, self.time_ls))
-
-    def _sample_ls(self, comp, vals):
-        mean, noise, amp2, max_ls = self.mean, self.noise, self.amp2, self.max_ls
-
-        def hypers_of(ls):
-            if np.any(ls < 0) or np.any(ls > max_ls):
-                return None
-            return (mean, noise, amp2, ls), ()
-        self.ls = util.slice_sample(self.ls, util.make_logprob(self._ll_obj, hypers_of), compwise=True)
-
-    def _sample_time_ls(self, comp, durs):
-        mean, noise, amp2, max_ls = self.time_mean, self.time_noise, self.time_amp2, self.time_max_ls
-
-        def hypers_of(ls):
-            if np.any(ls < 0) or np.any(ls > max_ls):
-                return None
-            return (mean, noise, amp2, ls), ()
-        self.time_ls = util.slice_sample(self.time_ls, util.make_logprob(self._ll_time, hypers_of), compwise=True)
-
-    def _sample_noisy(self, comp, vals):
-        vmax, vmin, ls = np.max(vals), np.min(vals), self.ls
-
-        def hypers_of(hypers):
-            mean, amp2, noise = hypers[0], hypers[1], hypers[2]
-            if mean > vmax or mean < vmin:
-                return None
-            if amp2 < 0 or noise < 0:
-                return None
-            return (mean, noise, amp2, ls), (
-                np.log(np.log(1 + (self.noise_scale / noise) ** 2)),
-                -0.5 * (np.log(amp2) / self.amp2_scale) ** 2)               # log(amp2), not log(sqrt(amp2)): PSEC:614
-        hypers = util.slice_sample(np.array([self.mean, self.amp2, self.noise]),
-                                   util.make_logprob(self._ll_obj, hypers_of), compwise=False)
-        self.mean, self.amp2, self.noise = hypers[0], hypers[1], hypers[2]
-
-    def _sample_time_noisy(self, comp, durs):
-        vmax, vmin, ls = np.max(durs), np.min(durs), self.time_ls
-
-        def hypers_of(hypers):
-            mean, amp2, noise = hypers[0], hypers[1], hypers[2]
-            if mean > vmax or mean < vmin:
-                return None
-            if amp2 < 0 or noise < 0:
-                return None
-            return (mean, noise, amp2, ls), (
-                np.log(np.log(1 + (self.time_noise_scale / noise) ** 2)),
-                -0.5 * (np.log(np.sqrt(amp2)) / self.time_amp2_scale) ** 2)   # PSEC:646
-        hypers = util.slice_sample(np.array([self.time_mean, self.time_amp2, self.time_noise]),
-                                   util.make_logprob(self._ll_time, hypers_of), compwise=False)
-        self.time_mean, self.time_amp2, self.time_noise = hypers[0], hypers[1], hypers[2]
-
-    def _sample_noiseless(self, comp, vals):
-        vmax, vmin, ls = np.max(vals), np.min(vals), self.ls
-
-        def hypers_of(hypers):
-            mean, amp2 = hypers[0], hypers[1]
-            if mean > vmax or mean < vmin:
-                return None
-            if amp2 < 0:
-                return None
-            return (mean, 1e-3, amp2, ls), (-0.5 * (np.log(amp2) / self.amp2_scale) ** 2,)
-        hypers = util.slice_sample(np.array([self.mean, self.amp2, self.noise]),
-                                   util.make_logprob(self._ll_obj, hypers_of), compwise=False)
-        self.mean, self.amp2, self.noise = hypers[0], hypers[1], 1e-3

@@ -20,6 +20,7 @@ import numpy as np
 import numpy.random as npr
 
 from spearmint_b200 import util
+from spearmint_b200.chooser._gp import LazyBackend
 from spearmint_b200.forest import draws
 
 
@@ -54,7 +55,7 @@ def resolve_max_features(max_features, D):
     return max(1, int(float(max_features) * D))
 
 
-class RandomForestEIChooserB200(object):
+class RandomForestEIChooserB200(LazyBackend):
 
     def __init__(self, n_trees=50, max_depth=None, min_samples_split=1, max_monkeys=7, max_features="auto", n_jobs=1,
                  random_state=None, device=None, backend=None):
@@ -64,13 +65,6 @@ class RandomForestEIChooserB200(object):
         self.max_features = _max_features(max_features)
         self.random_state = _none_or_int(random_state)
         self._device, self._backend = device, backend
-
-    @property
-    def backend(self):
-        if self._backend is None:
-            from spearmint_b200.backend import DeviceBackend
-            self._backend = DeviceBackend(device=self._device)
-        return self._backend
 
     def _fit(self, X, y):
         if not np.all(np.isfinite(y)):       # sklearn validates y before it draws the seeds

@@ -1035,18 +1035,27 @@ class LogLik(object):
         self.calls = 0
         self.launch_batches = 0
 
-    def batch(self, hypers):
-        """hypers: list of (mean, noise, amp2, ls).  Returns a float64 array; NaN marks a non-PD matrix."""
-        out = np.empty(len(hypers))
+    def _chunk(self, items):
+        """(HyperBatch, right-hand side on the device) of one launch batch of ``batch``'s items."""
+        return self.eng.hypers([(h[0], h[1], h[2], np.asarray(h[3], dtype=float)) for h in items], self.kind), self.y
+
+    def _set_rhs(self, B, hb, y, st):
+        """Writes each item's residual y - mean into the augmented row of its matrix."""
+        check(fn("smk_loglik_set_rhs", self.eng.dtype)(self.N, self.Npad, B, ptr(y), ptr(hb.mean), ptr(self.L), st),
+              "loglik_set_rhs")
+
+    def batch(self, items):
+        """items: list of (mean, noise, amp2, ls).  Returns a float64 array; NaN marks a non-PD matrix."""
+        out = np.empty(len(items))
         eng, dt, N, Npad = self.eng, self.eng.dtype, self.N, self.Npad
-        for b0 in range(0, len(hypers), self.max_batch):
-            hs = hypers[b0:b0 + self.max_batch]
-            B = len(hs)
-            hb = eng.hypers([(h[0], h[1], h[2], np.asarray(h[3], dtype=float)) for h in hs], self.kind)
+        for b0 in range(0, len(items), self.max_batch):
+            its = items[b0:b0 + self.max_batch]
+            B = len(its)
+            hb, y = self._chunk(its)
             st = eng.stream()
             check(fn("smk_cov_build_lower", dt)(KINDS[self.kind], N, self.D, B, ptr(self.X), ptr(hb.inv_ls),
                                                 ptr(hb.amp2), ptr(hb.noise), ptr(self.L), Npad, st), "cov_build")
-            check(fn("smk_loglik_set_rhs", dt)(N, Npad, B, ptr(self.y), ptr(hb.mean), ptr(self.L), st), "loglik_set_rhs")
+            self._set_rhs(B, hb, y, st)
             if self.fast:
                 check(_lib.lib().smk_potrf_loglik_f64(Npad, B, ptr(self.L), ptr(self.winv), self.ws_bytes, ptr(self.info),
                                                       self.use_graph, st), "potrf_loglik")
@@ -1062,8 +1071,8 @@ class LogLik(object):
             self.launch_batches += 1
         return out
 
-    def __call__(self, mean, noise, amp2, ls):
-        v = self.batch([(mean, noise, amp2, ls)])[0]
+    def __call__(self, *item):
+        v = self.batch([item])[0]
         if np.isnan(v):
             raise np.linalg.LinAlgError("leading minor of the array is not positive definite")
         return v
@@ -1148,39 +1157,14 @@ class LatentLogLik(LogLik):
         LogLik.__init__(self, eng, kind, comp, np.zeros(comp.shape[0]), max_batch)
         self.ls, self.noise = np.atleast_1d(np.asarray(ls, dtype=float)), float(noise)
 
-    def batch(self, items):
-        """items: list of (amp2, ff).  Returns a float64 array; NaN marks a non-PD matrix."""
-        out = np.empty(len(items))
-        eng, dt, N, Npad = self.eng, self.eng.dtype, self.N, self.Npad
-        for b0 in range(0, len(items), self.max_batch):
-            its = items[b0:b0 + self.max_batch]
-            B = len(its)
-            hb = eng.hypers([(0.0, self.noise, float(a), self.ls) for a, _ in its], self.kind)
-            y = eng.to_dev(np.vstack([np.ravel(f) for _, f in its]))
-            st = eng.stream()
-            check(fn("smk_cov_build_lower", dt)(KINDS[self.kind], N, self.D, B, ptr(self.X), ptr(hb.inv_ls),
-                                                ptr(hb.amp2), ptr(hb.noise), ptr(self.L), Npad, st), "cov_build")
-            check(fn("smk_loglik_set_rhs_batched", dt)(N, Npad, B, ptr(y), N, ptr(self.L), st), "loglik_set_rhs_batched")
-            if self.fast:
-                check(_lib.lib().smk_potrf_loglik_f64(Npad, B, ptr(self.L), ptr(self.winv), self.ws_bytes, ptr(self.info),
-                                                      self.use_graph, st), "potrf_loglik")
-            else:
-                check(fn("smk_potrf_lower_batched", dt)(Npad, B, ptr(self.L), ptr(self.winv), ptr(self.info), st), "potrf")
-            check(fn("smk_loglik_finish", dt)(N, Npad, B, ptr(self.L), ptr(self.out[0]), ptr(self.out[1]), st),
-                  "loglik_finish")
-            r = torch.cat([self.out[0, :B].double(), self.out[1, :B].double(), self.info[:B].double()]).cpu().numpy()
-            lp = -r[:B] - 0.5 * r[B:2 * B]
-            lp[r[2 * B:] != 0] = np.nan
-            out[b0:b0 + B] = lp
-            self.calls += B
-            self.launch_batches += 1
-        return out
+    def _chunk(self, items):
+        """items: (amp2, ff) pairs; each ff is its own right-hand side."""
+        hb = self.eng.hypers([(0.0, self.noise, float(a), self.ls) for a, _ in items], self.kind)
+        return hb, self.eng.to_dev(np.vstack([np.ravel(f) for _, f in items]))
 
-    def __call__(self, amp2, ff):
-        v = self.batch([(amp2, ff)])[0]
-        if np.isnan(v):
-            raise np.linalg.LinAlgError("leading minor of the array is not positive definite")
-        return v
+    def _set_rhs(self, B, hb, y, st):
+        check(fn("smk_loglik_set_rhs_batched", self.eng.dtype)(self.N, self.Npad, B, ptr(y), self.N, ptr(self.L), st),
+              "loglik_set_rhs_batched")
 
 
 class LatentFactor(object):

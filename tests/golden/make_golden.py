@@ -2,7 +2,7 @@
 """Generates tests/golden/*.npz by EXECUTING the reference (through oracle/ref_shim.py).
 
 Run in the build container only (needs /root/reference):
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py [name ...]        (no name: every case in CASES)
 Each .npz holds the exact inputs handed to the reference and the outputs it produced
 (float64), so the fixtures travel to the GPU box where the reference does not exist.
 """
@@ -184,9 +184,10 @@ def golden_logprob(name, D, N, kind, seed):
     print(name, "joint", len(out["noisy_joint_lp"]), "ls", len(out["noisy_ls_lp"]))
 
 
-def golden_psec(name, D, N, M, P, kind, S, seed, burnin=6):
+def golden_psec(name, D, N, M, P, kind, S, seed, burnin=6, noiseless=False):
     grid, values, durations, candidates, pending, complete = synth(D, N, M, P, seed)
-    ch = PSEC.init(tempfile.mkdtemp(), "covar=%s,mcmc_iters=%d,burnin=%d,grid_subset=4" % (kind, S, burnin))
+    ch = PSEC.init(tempfile.mkdtemp(), "covar=%s,mcmc_iters=%d,burnin=%d,grid_subset=4,noiseless=%d" % (
+        kind, S, burnin, int(noiseless)))
     np.random.seed(seed)
     ret = ch.next(grid, values, durations, candidates, pending, complete)
     comp, cand, pend = grid[complete], grid[candidates], grid[pending]
@@ -207,7 +208,8 @@ def golden_psec(name, D, N, M, P, kind, S, seed, burnin=6):
         gg.append(g)
     m, n, a, l = pack_hypers(hs)
     tm, tn, ta, tl = pack_hypers(ths)
-    out = dict(kind=kind, S=S, seed=seed, burnin=burnin, grid=grid, values=values, durations=durations,
+    out = dict(kind=kind, S=S, seed=seed, burnin=burnin, noiseless=int(noiseless), grid=grid, values=values,
+               durations=durations,
                candidates=candidates, pending=pending, complete=complete,
                hs_mean=m, hs_noise=n, hs_amp2=a, hs_ls=l,
                ths_mean=tm, ths_noise=tn, ths_amp2=ta, ths_ls=tl, n_time_samples=len(ths),
@@ -220,28 +222,39 @@ def golden_psec(name, D, N, M, P, kind, S, seed, burnin=6):
     print(name, "next ->", out["next_index"], out["next_is_tuple"])
 
 
-def golden_gpei(name, D, N, M, P, seed):
+def golden_gpei(name, D, N, M, P, seed, noiseless=False):
+    """GPEIChooser: the proposal; with ``noiseless`` also the hyper-parameters the chain ends on."""
     grid, values, durations, candidates, pending, complete = synth(D, N, M, P, seed)
-    ch = GPEI.init(tempfile.mkdtemp(), "mcmc_iters=4")
+    ch = GPEI.init(tempfile.mkdtemp(), "mcmc_iters=4" + (",noiseless=1" if noiseless else ""))
     np.random.seed(seed)
     ret = ch.next(grid, values, durations, candidates, pending, complete)
     out = dict(grid=grid, values=values, durations=durations, candidates=candidates, pending=pending,
                complete=complete, seed=seed, next_index=int(ret))
+    if noiseless:
+        out.update(noiseless=1, mean=ch.mean, noise=ch.noise, amp2=ch.amp2, ls=ch.ls)
     np.savez_compressed(os.path.join(HERE, name + ".npz"), **out)
     print(name, "next ->", int(ret))
 
 
+CASES = {
+    "kernels":            lambda n: golden_kernels(),
+    #                                  name  D   N    M   P  kind        S noiseless seed
+    "opt_branin2d":       lambda n: golden_opt(n, 2, 20, 300, 0, "Matern52", 4, False, 1),
+    "opt_d8_m52":         lambda n: golden_opt(n, 8, 64, 400, 0, "Matern52", 4, True, 2),
+    "opt_d8_m52_pend":    lambda n: golden_opt(n, 8, 48, 300, 3, "Matern52", 3, True, 3),
+    "opt_d5_ardse":       lambda n: golden_opt(n, 5, 40, 300, 0, "ARDSE", 3, False, 4),
+    "opt_d4_m32_pend":    lambda n: golden_opt(n, 4, 32, 200, 2, "Matern32", 3, False, 5),
+    "opt_d3_se":          lambda n: golden_se(n, 3, 24, 200, 2, 6),
+    "opt_d1_m52":         lambda n: golden_opt(n, 1, 12, 100, 1, "Matern52", 2, False, 7),
+    "logprob_d6":         lambda n: golden_logprob(n, 6, 40, "Matern52", 8),
+    "psec_d4":            lambda n: golden_psec(n, 4, 40, 300, 0, "Matern52", 3, 9),
+    "psec_d3_pend":       lambda n: golden_psec(n, 3, 30, 200, 2, "Matern52", 2, 10),
+    "psec_d3_noiseless":  lambda n: golden_psec(n, 3, 30, 200, 2, "Matern52", 2, 13, noiseless=True),
+    "gpei_d3":            lambda n: golden_gpei(n, 3, 25, 200, 2, 12),
+    "gpei_d3_noiseless":  lambda n: golden_gpei(n, 3, 25, 200, 2, 14, noiseless=True),
+}
+
+
 if __name__ == "__main__":
-    golden_kernels()
-    #           name              D   N    M   P  kind        S noiseless seed
-    golden_opt("opt_branin2d",    2, 20, 300, 0, "Matern52", 4, False, 1)
-    golden_opt("opt_d8_m52",      8, 64, 400, 0, "Matern52", 4, True, 2)
-    golden_opt("opt_d8_m52_pend", 8, 48, 300, 3, "Matern52", 3, True, 3)
-    golden_opt("opt_d5_ardse",    5, 40, 300, 0, "ARDSE", 3, False, 4)
-    golden_opt("opt_d4_m32_pend", 4, 32, 200, 2, "Matern32", 3, False, 5)
-    golden_se("opt_d3_se",        3, 24, 200, 2, 6)
-    golden_opt("opt_d1_m52",      1, 12, 100, 1, "Matern52", 2, False, 7)
-    golden_logprob("logprob_d6",  6, 40, "Matern52", 8)
-    golden_psec("psec_d4",        4, 40, 300, 0, "Matern52", 3, 9)
-    golden_psec("psec_d3_pend",   3, 30, 200, 2, "Matern52", 2, 10)
-    golden_gpei("gpei_d3",        3, 25, 200, 2, 12)
+    for name in sys.argv[1:] or list(CASES):       # e.g. make_golden.py gpei_d3_noiseless
+        CASES[name](name)
