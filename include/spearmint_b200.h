@@ -137,6 +137,13 @@ int smk_predict_f64(int kind, int N, int Npad, int M, int D, int S, const double
                     const double* inv_ls, const double* amp2, const double* mean, const double* L,
                     const double* winv, const double* alpha, double* mu, double* var, int ldm,
                     void* workspace, size_t workspace_bytes, void* stream);
+/* (4-mma) smk_predict_f64 on the fp64 tensor cores (mma.sync.m8n8k4.f64): same arguments, outputs, error codes and
+ * workspace (smk_predict_workspace_bytes(8, Npad)).  The off-diagonal update and the diagonal-block solve of every row
+ * block run on DMMA, the cross-covariance on DFMA; results differ from smk_predict_f64 only by summation order.   */
+int smk_predict_mma_f64(int kind, int N, int Npad, int M, int D, int S, const double* X, const double* C,
+                        const double* inv_ls, const double* amp2, const double* mean, const double* L,
+                        const double* winv, const double* alpha, double* mu, double* var, int ldm,
+                        void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- (4-tc) fused predict on the tensor cores (wgmma + TMA, register accumulators; float32 in/out, 3 x FP16 split products
  *      with exact power-of-two operand scaling, fp32 accumulation)

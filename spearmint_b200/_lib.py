@@ -71,6 +71,7 @@ SIGNATURES = {
     "smk_linv_pack_f16": ([_i, _i, _p, _p, _p, _p, _p, _p], _i),
     "smk_predict_tc_f32": ([_i] * 6 + [_p] * 9 + [_i, _p, _p, _i, _p, _sz, _p, _i, _p, _p, _p, _i, _p], _i),
     "smk_predict_tc_pregen_f32": ([_i] * 6 + [_p] * 5 + [_sz, _i, _p], _i),
+    "smk_predict_mma_f64": ([_i] * 6 + [_p] * 10 + [_i, _p, _sz, _p], _i),
     "smk_lower_matvec_f64": ([_i, _i, _p, _p, _p, _p], _i),
     "smk_forest_workspace_bytes": ([_i, _i, _i], _sz),
     "smk_forest_fit_f64": ([_i] * 3 + [_p] * 4 + [_i] * 4 + [_p] * 7 + [_p, _sz, _p], _i),

@@ -35,13 +35,24 @@ class _GridState(object):
 class DeviceBackend(object):
     name = "b200"
 
-    def __init__(self, device=None, refine_dtype="float64"):
+    def __init__(self, device=None, refine_dtype="float64", grid_dtype="float32"):
+        """``grid_dtype``: precision of the grid pass (grid_state, ei_matrix, top_mean_ei, constrained_ei_matrix,
+        constraint_predict).  "float32" is the production chain; "float64" runs it on the float64 engine (the reference's
+        precision, with the prediction on the fp64 tensor cores from f64_mma_min_n on) and needs no deep-tail re-scoring."""
+        if grid_dtype not in ("float32", "float64"):
+            raise ValueError("grid_dtype must be float32 or float64, got %r" % (grid_dtype,))
         if device is None and torch.cuda.is_available():
             rank, world = parallel.world()
             device = "cuda:%d" % (torch.cuda.current_device() if world == 1 else rank % torch.cuda.device_count())
         self.eng32 = GPEIEngine(device=device, dtype=torch.float32)
         self.eng64 = GPEIEngine(device=device, dtype=torch.float64)
         self.refine_eng = self.eng64 if refine_dtype == "float64" else self.eng32
+        self.grid_dtype = grid_dtype
+
+    @property
+    def grid_eng(self):
+        """The engine of the grid pass: the float64 one with grid_dtype="float64", else the float32 one."""
+        return self.eng64 if getattr(self, "grid_dtype", "float32") == "float64" else self.eng32
 
     # ---- f2
     def loglik(self, kind, comp, vals):
@@ -60,7 +71,7 @@ class DeviceBackend(object):
     def grid_state(self, kind, hyper_samples, comp, pend, vals, normals=None, time_hyper_samples=None,
                    durs_log=None):
         """Factors all (local) hyper-samples once; reused by both grid passes of next() (OPT:269, OPT:293)."""
-        eng = self.eng32
+        eng = self.grid_eng
         rank, world = parallel.world()
         S = len(hyper_samples)
         mine = parallel.shard(S, rank, world)
@@ -93,7 +104,7 @@ class DeviceBackend(object):
     def _local(self, st, cand, want_matrix):
         """This rank's EI (matrix and sum over its hyper-samples).  Every rank ends with the same single
         agree_on_error() collective, whatever path it took (resident factors, chunked, empty shard)."""
-        eng = self.eng32
+        eng = self.grid_eng
         ldm = _ceil(cand.shape[0], 128)
         err, ei, ei_sum = None, None, None
         if not st.hs:
@@ -118,9 +129,10 @@ class DeviceBackend(object):
         return ei, ei_sum
 
     def _tail_fix(self, st, cand, ei, ei_sum, M):
-        """float64 re-evaluation of the short-list when the pass is in the deep-tail regime (engine.tail_fix)."""
+        """float64 re-evaluation of the short-list when the pass is in the deep-tail regime (engine.tail_fix); a float64
+        pass has nothing to re-evaluate (the float64 engine's tail_fix returns at once)."""
         comp, pend, vals, normals, durs_log = st.args
-        return self.eng32.tail_fix(st.kind, st.hs, st.S, comp, pend, cand, vals, normals, st.ths, durs_log, ei, ei_sum, M,
+        return self.grid_eng.tail_fix(st.kind, st.hs, st.S, comp, pend, cand, vals, normals, st.ths, durs_log, ei, ei_sum, M,
                                    reduce_fn=parallel.allreduce_sum_)
 
     def ei_matrix(self, st, cand):
@@ -132,7 +144,7 @@ class DeviceBackend(object):
             return ei[:, :M].t().contiguous().double().cpu().numpy()
         parallel.allreduce_sum_(ei_sum)
         self._tail_fix(st, cand, ei, ei_sum, M)      # the same decision on every rank (global sum); local columns fixed
-        full = torch.zeros((st.S, _ceil(M, 128)), dtype=torch.float64, device=self.eng32.device)
+        full = torch.zeros((st.S, _ceil(M, 128)), dtype=torch.float64, device=self.grid_eng.device)
         if ei is not None:
             full[st.mine] = ei
         parallel.allreduce_sum_(full)                # columns are disjoint across ranks
@@ -143,7 +155,7 @@ class DeviceBackend(object):
         _, ei_sum = self._local(st, cand, False)
         parallel.allreduce_sum_(ei_sum)              # the single exchange of the path (SURVEY 8e)
         self._tail_fix(st, cand, None, ei_sum, M)    # deep-tail passes: exact float64 ranking of the short-list
-        idx, _ = self.eng32.topk(ei_sum, M, k)       # argsort / argmax of the mean == of the sum
+        idx, _ = self.grid_eng.topk(ei_sum, M, k)    # argsort / argmax of the mean == of the sum
         out = idx.cpu().numpy().astype(int)
         if np.any(out < 0):                          # every score NaN: the reference's argmax would return index 0 of NaNs
             raise FloatingPointError("EI is NaN for every candidate (non-finite hyper-parameters or inputs)")
@@ -155,7 +167,7 @@ class DeviceBackend(object):
         """(M, S) float64 numpy: GPConstrainedEIChooser.ei_over_hypers (CONS:450-468).  Sample PAIRS -- objective sample s
         with constraint sample s -- are sharded round-robin over ranks, per-sample fantasy normals (S,P,F) with them; the
         per-candidate sum is all-reduced once (it decides the deep-tail re-evaluation), the disjoint columns once."""
-        eng = self.eng32
+        eng = self.grid_eng
         rank, world = parallel.world()
         S, M = len(hyper_samples), cand.shape[0]
         ldm = _ceil(M, 128)
@@ -188,7 +200,7 @@ class DeviceBackend(object):
 
     def constraint_predict(self, kind, chyper, ff, comp, cand):
         """Phi(gain m_c) at ``cand`` for ONE constraint sample (pred_constraint_voilation, CONS:425-447), (M,) numpy."""
-        eng = self.eng32
+        eng = self.grid_eng
         p, _ = eng.constraint_prob_device(kind, [chyper], ff, comp, None, eng.to_dev(cand))
         return p[0, :cand.shape[0]].cpu().numpy()
 

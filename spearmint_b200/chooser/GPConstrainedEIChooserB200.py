@@ -19,7 +19,8 @@ no violation has been seen, the refinement does not; the refinement takes its va
 sums over fantasies; the second grid pass scores the refined AND the unrefined short-list; the jitter cloud centres on
 ``argmin`` of all values (the first NaN if there is one).  Waived: ``pending_samples`` is cast to int, a truthy
 ``visualize2D`` raises NotImplementedError (no plotting), ``constraint_gain`` is written to the pickle, factorisations
-whose result the reference never uses are skipped.  Extra optional keys: ``device``, ``refine_dtype``, ``state_name``.
+whose result the reference never uses are skipped.  Extra optional keys: ``device``, ``refine_dtype``, ``grid_dtype``,
+``state_name``.
 """
 import math
 
@@ -74,9 +75,9 @@ class GPConstrainedEIChooserB200(GPChooser):
 
     def __init__(self, expt_dir, covar="Matern52", mcmc_iters=20, pending_samples=100, noiseless=False, burnin=100,
                  grid_subset=20, constraint_violating_value=np.inf, verbosity=0, visualize2D=False, device=None,
-                 refine_dtype="float64", state_name=None, backend=None):
+                 refine_dtype="float64", state_name=None, backend=None, grid_dtype="float32"):
         GPChooser.__init__(self, expt_dir, covar, mcmc_iters, pending_samples, noiseless, state_name, device, backend,
-                           refine_dtype)
+                           refine_dtype, grid_dtype)
         if visualize2D:      # an arg string hands over a non-empty str, which the reference treats as true (CONS:308)
             raise NotImplementedError("visualize2D: the 2-D contour plots of the reference are not provided")
         self.burnin = int(burnin)

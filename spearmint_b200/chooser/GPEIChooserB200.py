@@ -25,8 +25,9 @@ class GPEIChooserB200(GPChooser):
     prior = GPPrior(max_ls=2)
 
     def __init__(self, expt_dir, covar="Matern52", mcmc_iters=10, pending_samples=100, noiseless=False,
-                 device=None, state_name=None, backend=None):
-        GPChooser.__init__(self, expt_dir, covar, mcmc_iters, pending_samples, noiseless, state_name, device, backend)
+                 device=None, state_name=None, backend=None, grid_dtype="float32"):
+        GPChooser.__init__(self, expt_dir, covar, mcmc_iters, pending_samples, noiseless, state_name, device, backend,
+                           grid_dtype=grid_dtype)
 
     def dump_hypers(self):
         if self.D == -1:

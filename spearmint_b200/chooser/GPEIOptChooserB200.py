@@ -13,7 +13,8 @@ evaluation is a hand-written sm_90a kernel behind the C ABI (``spearmint_b200.ba
   * L-BFGS-B refinement    : scipy on the host, (f, g) from the GPU with the S factors cached         [f1]
                              (the reference re-factors K for every sample at every evaluation)
 ``use_multiprocessing`` is accepted and ignored: a forked pool cannot share a CUDA context, and with cached
-factors the 20 refinements are cheap.  Extra optional keys: ``device``, ``refine_dtype``, ``state_name``.
+factors the 20 refinements are cheap.  Extra optional keys: ``device``, ``refine_dtype``, ``grid_dtype``,
+``state_name``.
 """
 import time
 
@@ -36,9 +37,9 @@ class GPEIOptChooserB200(GPChooser):
 
     def __init__(self, expt_dir, covar="Matern52", mcmc_iters=10, pending_samples=100, noiseless=False, burnin=100,
                  grid_subset=20, use_multiprocessing=True, device=None, refine_dtype="float64", state_name=None,
-                 backend=None):
+                 backend=None, grid_dtype="float32"):
         GPChooser.__init__(self, expt_dir, covar, mcmc_iters, pending_samples, noiseless, state_name, device, backend,
-                           refine_dtype)
+                           refine_dtype, grid_dtype)
         self.burnin = int(burnin)
         self.needs_burnin = True
         self.grid_subset = int(grid_subset)

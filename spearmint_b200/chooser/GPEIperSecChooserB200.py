@@ -29,9 +29,9 @@ class GPEIperSecChooserB200(GPChooser):
     time_prior = GPPrior(max_ls=10, amp2_prior_on_std=True)      # log(sqrt(amp2)) prior: PSEC:646
 
     def __init__(self, expt_dir, covar="Matern52", mcmc_iters=10, pending_samples=100, noiseless=False, burnin=100,
-                 grid_subset=20, device=None, refine_dtype="float64", state_name=None, backend=None):
+                 grid_subset=20, device=None, refine_dtype="float64", state_name=None, backend=None, grid_dtype="float32"):
         GPChooser.__init__(self, expt_dir, covar, mcmc_iters, pending_samples, noiseless, state_name, device, backend,
-                           refine_dtype)
+                           refine_dtype, grid_dtype)
         self.burnin = int(burnin)
         self.needs_burnin = True
         self.grid_subset = int(grid_subset)

@@ -24,6 +24,7 @@ from spearmint_b200 import util
 from spearmint_b200.locker import Locker
 
 COVARS = ("SE", "ARDSE", "Matern32", "Matern52")     # the stationary kernels of gp.py:87-127
+GRID_DTYPES = ("float32", "float64")                 # precision of the grid pass (DeviceBackend grid_dtype)
 
 
 class GPPrior(object):
@@ -115,12 +116,14 @@ class LazyBackend(object):
     """The ``backend`` property: a DeviceBackend made on first use (raises if there is no GPU), unless one was given."""
     _device = _backend = None
     _refine_dtype = "float64"
+    _grid_dtype = "float32"
 
     @property
     def backend(self):
         if self._backend is None:
             from spearmint_b200.backend import DeviceBackend
-            self._backend = DeviceBackend(device=self._device, refine_dtype=self._refine_dtype)
+            self._backend = DeviceBackend(device=self._device, refine_dtype=self._refine_dtype,
+                                          grid_dtype=self._grid_dtype)
         return self._backend
 
 
@@ -129,9 +132,11 @@ class GPChooser(LazyBackend):
     handle while a chain is being sampled."""
 
     def __init__(self, expt_dir, covar, mcmc_iters, pending_samples, noiseless, state_name, device, backend,
-                 refine_dtype="float64"):
+                 refine_dtype="float64", grid_dtype="float32"):
         if covar not in COVARS:
             raise AttributeError("module 'spearmint.gp' has no attribute '%s'" % covar)   # getattr(gp, covar)
+        if grid_dtype not in GRID_DTYPES:
+            raise ValueError("grid_dtype must be one of %s, got %r" % ("/".join(GRID_DTYPES), grid_dtype))
         self.covar = covar
         self.locker = Locker()
         name = state_name if state_name else self.__module__
@@ -142,7 +147,7 @@ class GPChooser(LazyBackend):
         self.D = -1
         self.hyper_iters = 1
         self.noiseless = bool(int(noiseless))
-        self._device, self._refine_dtype, self._backend = device, refine_dtype, backend
+        self._device, self._refine_dtype, self._grid_dtype, self._backend = device, refine_dtype, grid_dtype, backend
         self._loglik = None
 
     def _ll(self, comp, vals):

@@ -104,6 +104,8 @@ int predict_tc(int, int, int, int, int, int, const float*, const float*, const f
 int predict_tc_pregen(int, int, int, int, int, int, const float*, const float*, const float*, const float*, void*, size_t,
                       int, cudaStream_t);
 size_t predict_workspace_bytes_any(int, int);
+int predict_mma_f64(int, int, int, int, int, int, const double*, const double*, const double*, const double*, const double*,
+                    const double*, const double*, const double*, double*, double*, int, void*, size_t, cudaStream_t);
 size_t potrf_ll_workspace_bytes(int, int);
 template <typename T>
 int sobol_generate(int, long, long, const uint32_t*, T*, cudaStream_t);
@@ -229,6 +231,13 @@ int smk_predict_f64(int kind, int N, int Npad, int M, int D, int S, const double
                     const double* winv, const double* alpha, double* mu, double* var, int ldm, void* workspace,
                     size_t workspace_bytes, void* stream) {
   return predict<double>(kind, N, Npad, M, D, S, X, C, inv_ls, amp2, mean, L, winv, alpha, mu, var, ldm, workspace,
+                         workspace_bytes, ST(stream));
+}
+int smk_predict_mma_f64(int kind, int N, int Npad, int M, int D, int S, const double* X, const double* C,
+                        const double* inv_ls, const double* amp2, const double* mean, const double* L,
+                        const double* winv, const double* alpha, double* mu, double* var, int ldm, void* workspace,
+                        size_t workspace_bytes, void* stream) {
+  return predict_mma_f64(kind, N, Npad, M, D, S, X, C, inv_ls, amp2, mean, L, winv, alpha, mu, var, ldm, workspace,
                          workspace_bytes, ST(stream));
 }
 

@@ -248,6 +248,9 @@ class GPEIEngine(object):
         # ill-conditioned problems small N goes with (C2 / C4: 1.5e-3 against 8e-3 ... 1.2e-2 of max EI, DESIGN.md section 6)
         # and at that size it costs milliseconds.
         self.tc_min_n = int(os.environ.get("SMK_TC_MIN_N", "2048"))
+        # float64 engine: factors of at least f64_mma_min_n observations predict on the fp64 tensor cores
+        # (smk_predict_mma_f64, DMMA), smaller ones on the SIMT kernel (smk_predict_f64, DFMA) -- DESIGN.md section 5
+        self.f64_mma_min_n = int(os.environ.get("SMK_F64_MMA_MIN_N", "128"))
         # opt-in accuracy guard of the tensor-core chain (csrc/guard.cu, _guarded_impl): a hyper-sample whose ESTIMATED EI
         # error exceeds this fraction of its EI scale is re-evaluated in float64.  The estimate is conservative (it
         # over-predicts the actual error), so it is off by default (0) and meant for users whose problems are both large
@@ -395,6 +398,11 @@ class GPEIEngine(object):
             return "tc"
         return "simt"
 
+    def predict_kernel_for(self, n):
+        """("mma" | "simt") blocked-substitution predict kernel for a factor of n observations: the float64 engine runs the
+        fp64 tensor-core kernel from f64_mma_min_n on, everything else the SIMT kernel."""
+        return "mma" if self.dtype == torch.float64 and n >= self.f64_mma_min_n else "simt"
+
     def cov(self, kind, hb, X, Y=None):
         """Batched chooser.cov (OPT:207-212): returns [S][N][N] (self, jitter included, no noise) or [S][N][M]."""
         N, D = X.shape
@@ -458,9 +466,10 @@ class GPEIEngine(object):
             return mu, var, ldm
         nb = _lib.lib().smk_predict_workspace_bytes(self.esize, fac.Npad)
         ws = self.workspace(nb)
-        check(fn("smk_predict", dt)(KINDS[kind], fac.N, fac.Npad, M, fac.D, hb.S, ptr(fac.X), ptr(C_dev),
-                                    ptr(hb.inv_ls), ptr(hb.amp2), ptr(hb.mean), ptr(fac.L), ptr(fac.winv),
-                                    ptr(alpha), ptr(mu), ptr(var), ldm, ptr(ws), nb, self.stream()), "predict")
+        entry = _lib.lib().smk_predict_mma_f64 if self.predict_kernel_for(fac.N) == "mma" else fn("smk_predict", dt)
+        check(entry(KINDS[kind], fac.N, fac.Npad, M, fac.D, hb.S, ptr(fac.X), ptr(C_dev), ptr(hb.inv_ls), ptr(hb.amp2),
+                    ptr(hb.mean), ptr(fac.L), ptr(fac.winv), ptr(alpha), ptr(mu), ptr(var), ldm, ptr(ws), nb,
+                    self.stream()), "predict")
         return mu, var, ldm
 
     def cross_mean(self, kind, fac, C_dev, alpha, F):
