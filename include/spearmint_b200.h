@@ -304,7 +304,8 @@ int smk_forest_predict_ei_f64(int M, int D, int T, int ldn, const float* C, cons
 /* ---- (6) selection: argsort(mean)[-k:] and argmax(mean)   (OPT:270-271, OPT:294)
  * score: [M].  idx_out[k]: indices of the k largest scores in ASCENDING score order (so
  * idx_out[k-1] is the argmax; ties resolved towards the lower index, numpy's first-max rule).
- * workspace: smk_topk_workspace_bytes(M, k).                                                    */
+ * NaN scores are never selected: with fewer than k non-NaN scores the first slots get index -1 and value -inf.
+ * k <= 256 and k <= M (else -2).  workspace: smk_topk_workspace_bytes(M, k) (else -6).              */
 size_t smk_topk_workspace_bytes(int M, int k);
 int smk_topk_f32(int M, int k, const float* score, int* idx_out, float* val_out,
                  void* workspace, size_t workspace_bytes, void* stream);

@@ -157,8 +157,9 @@ class DeviceBackend(object):
         self._tail_fix(st, cand, None, ei_sum, M)    # deep-tail passes: exact float64 ranking of the short-list
         idx, _ = self.grid_eng.topk(ei_sum, M, k)    # argsort / argmax of the mean == of the sum
         out = idx.cpu().numpy().astype(int)
-        if np.any(out < 0):                          # every score NaN: the reference's argmax would return index 0 of NaNs
-            raise FloatingPointError("EI is NaN for every candidate (non-finite hyper-parameters or inputs)")
+        if np.any(out < 0):                          # fewer than k non-NaN scores (the reference would rank NaNs)
+            raise FloatingPointError("EI is NaN for more than %d of %d candidates (non-finite hyper-parameters or "
+                                     "inputs)" % (M - k, M))
         return out
 
     # ---- constrained EI (CONS = chooser/GPConstrainedEIChooser.py)

@@ -19,7 +19,11 @@ __device__ __forceinline__ double ei_one(double best, double m, double v) {
   const double u = (best - m) / s;
   const double cdf = 0.5 * erfc(-u * 0.7071067811865476);
   const double pdf = 0.3989422804014327 * exp(-0.5 * u * u);
-  return s * (u * cdf + pdf);
+  // below u ~ -37.5 Phi and phi are denormal and u Phi + phi can round to a few denormal ulps below zero; EI is >= 0
+  // (written so that a NaN stays NaN).  Only the sweeps use ei_one; the EI-gradient kernels of the refinement (grad.cu)
+  // keep their own unclamped formula, so the two can differ by those denormal ulps deep in the tail.
+  const double e = s * (u * cdf + pdf);
+  return (e < 0.0) ? 0.0 : e;
 }
 
 // float32 moments (the grid path): the expression is evaluated in float32 wherever that is exact enough -- u > -4, where

@@ -503,7 +503,9 @@ class GPEIEngine(object):
     def topk(self, score, M, k):
         """Indices of the k largest scores, ascending (argsort(score)[-k:], OPT:270; [-1] is the argmax, OPT:294).
         The device selection handles k <= 256 per call; larger k (the reference accepts any grid_subset) takes several
-        rounds, each masking what the previous ones took."""
+        rounds, each masking what the previous ones took.  NaN scores are never selected: with fewer than k non-NaN
+        scores the first slots hold index -1 (value -inf), as in one call of smk_topk_*: backend.top_mean_ei raises on
+        it, the forest's argmax maps it to 0, and tail_fix never ranks a sum that holds a NaN."""
         dt = score.dtype                      # EI scores are float64 (see ei_sweep)
         K = 256
         if k <= K:
@@ -517,7 +519,10 @@ class GPEIEngine(object):
                 i, v = self._topk_once(work, M, kk)           # ascending
                 parts_i.append(i)
                 parts_v.append(v)
-                work[i.long()] = float("-inf")
+                # NaN, not -inf: the kernel never selects NaN, while a -inf mark could be taken again by a later round
+                # (fewer non-NaN scores than k, or genuine -inf scores).  An index -1 means every non-NaN score is taken
+                # already, so clamping it to 0 masks nothing that is still selectable.
+                work[i.long().clamp(min=0)] = float("nan")
                 left -= kk
             idx = torch.cat(parts_i[::-1])                   # later rounds hold smaller scores
             val = torch.cat(parts_v[::-1])

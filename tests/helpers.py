@@ -1,10 +1,12 @@
-"""Shared helpers of the tests: golden fixture loading, the inputs of the EI grid pass built as Factor builds them, and
-the host-side measures of a factorisation's error."""
+"""Shared helpers of the tests: golden fixture loading, the inputs of the EI grid pass built as Factor builds them, the
+host-side measures of a factorisation's error, and the float64 kernel references with their a-priori bounds."""
 import os
 
 import numpy as np
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+U32, U64 = 2.0 ** -24, 2.0 ** -53          # unit roundoff of float32 and float64
+GEN_EVAL_U = 24.0                          # kernel evaluation + scaling + fp16 pair of one generator element, units of u amp2
 
 OPT_CASES = ["opt_branin2d", "opt_d8_m52", "opt_d8_m52_pend", "opt_d5_ardse", "opt_d4_m32_pend",
              "opt_d3_se", "opt_d1_m52"]
@@ -135,6 +137,74 @@ def factor_path(path, A, Np):
                                         nb_t, st), "trtri_split")
     out["info"] = info.cpu().numpy()           # read back: nothing of this call is in flight afterwards
     return out
+
+
+# ---------------------------------------------------------------------------------------------------- kernel references
+def kern(kind, r2):
+    """k(r2) of the four kernel kinds (GP:87-127), in the precision of r2."""
+    if kind in ("SE", "ARDSE"):
+        return np.exp(-0.5 * r2)
+    r = np.sqrt(r2)
+    if kind == "Matern32":
+        a = np.sqrt(3.0) * r
+        return (1.0 + a) * np.exp(-a)
+    a = np.sqrt(5.0) * r
+    return (1.0 + a + (5.0 / 3.0) * r2) * np.exp(-a)
+
+
+def dkern(kind, r2):
+    """|dk / dr2|."""
+    if kind in ("SE", "ARDSE"):
+        return 0.5 * np.exp(-0.5 * r2)
+    r = np.sqrt(r2)
+    if kind == "Matern32":
+        return 1.5 * np.exp(-np.sqrt(3.0) * r)
+    return (5.0 / 6.0) * (1.0 + np.sqrt(5.0) * r) * np.exp(-np.sqrt(5.0) * r)
+
+
+def gen_bound(kind, r2, nc, nx, D, a2, u, eval_u=GEN_EVAL_U):
+    """A-priori bound of one element amp2 k(r2) of a SIMT generator that scales both points (c s, x s, rounded once each),
+    takes their difference (rounded once) and accumulates its square over d with D fused multiply-adds: each difference
+    is off by at most 2 u (|c s| + |x s|), its square by 4 u |Delta_d| (|c_d| + |x_d|) s_d, and the D fused multiply-adds
+    add at most (D + 2) u r2.  By Cauchy-Schwarz the sum over d is at most 4 u sqrt(r2) (|c s| + |x s|) + (D + 2) u r2,
+    which moves k by |dk/dr2| times that.  On top, eval_u u amp2 for the evaluation itself (sqrt and exp at most 2 ulp
+    each, the rounding of their arguments at most 2.3 u of k, three roundings of the polynomial, the amp2 product; 24
+    also covers the fp16 pair of the tensor-core operand).  nc, nx: the norms |c s|, |x s| broadcast against r2."""
+    dr2 = 4.0 * np.sqrt(r2) * (nc + nx) + (D + 2.0) * r2
+    return u * a2 * (eval_u + 1.01 * dkern(kind, r2) * dr2)
+
+
+class Worst(object):
+    """The largest value per key, recorded once at the end of a test."""
+
+    def __init__(self, rec):
+        self.rec, self.v = rec, {}
+
+    def __call__(self, key, val):
+        self.v[key] = max(self.v.get(key, 0.0), float(val))
+
+    def flush(self):
+        for k, v in sorted(self.v.items()):
+            self.rec(k, v)
+
+
+def same(a, b):
+    """Bit for bit, NaN sentinels included."""
+    return a.shape == b.shape and np.array_equal(a, b, equal_nan=True)
+
+
+def frac(err, bound, what):
+    """max err / bound, every entry within its bound (an entry whose bound is 0 must be exact)."""
+    err = np.atleast_1d(np.asarray(err, dtype=np.float64))       # argwhere of a 0-d array finds nothing
+    bound = np.broadcast_to(np.asarray(bound, dtype=np.float64), err.shape)
+    assert np.all(np.isfinite(err)), "%s: non-finite entries" % what
+    zero = bound == 0
+    assert not np.any(err[zero]), "%s: an entry with a zero bound is not exact" % what
+    f = float((err[~zero] / bound[~zero]).max()) if np.any(~zero) else 0.0
+    bad = np.argwhere(err > bound)
+    assert bad.size == 0, "%s: %d entries above the bound, first %s, worst %.3g x the bound" % (what, len(bad),
+                                                                                              bad[0].tolist(), f)
+    return f
 
 
 def check_rows(N, Npad, rs, nb=NB):

@@ -36,16 +36,16 @@ import numpy as np
 import pytest
 import scipy.linalg as spla
 
-from tests.helpers import cov_inputs, cur_stream, data, factor_path, lib, synth_hypers
+from tests.helpers import GEN_EVAL_U, U32, U64, Worst, cov_inputs, cur_stream, data, factor_path, gen_bound, lib, \
+    synth_hypers
+from tests.helpers import dkern as _dkern, frac as _frac, kern as _kern, same as _same
 
 gpu = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-U32, U64 = 2.0 ** -24, 2.0 ** -53
 BM, BN = 128, 256                  # candidate tile, row group of the tensor-core GEMM
 PROBLEMS = (("Matern52", 32), ("Matern52", 8), ("SE", 3))       # the bench's problem, the smooth D = 8 one, SE D = 3
 NOISES = (1e-2, 1e-3, 1e-4)
-GEN_EVAL_U = 24.0                  # kernel evaluation + scaling + fp16 pair of one generator element, units of u amp2
 
 
 def _npad(N):
@@ -69,35 +69,11 @@ def _gemm_u(Np):
 
 
 # ---------------------------------------------------------------------------------------------------- host references
-def _kern(kind, r2):
-    if kind in ("SE", "ARDSE"):
-        return np.exp(-0.5 * r2)
-    r = np.sqrt(r2)
-    if kind == "Matern32":
-        a = np.sqrt(3.0) * r
-        return (1.0 + a) * np.exp(-a)
-    a = np.sqrt(5.0) * r
-    return (1.0 + a + (5.0 / 3.0) * r2) * np.exp(-a)
-
-
-def _dkern(kind, r2):
-    """|dk / dr2|."""
-    if kind in ("SE", "ARDSE"):
-        return 0.5 * np.exp(-0.5 * r2)
-    r = np.sqrt(r2)
-    if kind == "Matern32":
-        return 1.5 * np.exp(-np.sqrt(3.0) * r)
-    return (5.0 / 6.0) * (1.0 + np.sqrt(5.0) * r) * np.exp(-np.sqrt(5.0) * r)
-
-
 def _kx_ref(P, C, s, tc_gen=False, u=U32):
     """amp2 k(X, C) [m][N] in float64 on the device's float32 operands, and the a-priori bound of each element.
 
-    SIMT generator (kxt_kernel; the same form holds for the fused generators of predict.cu and cross_mean): the scaled
-    coordinates c s, -x s are rounded once each and their sum once, so each difference is off by at most 2 u (|c s| +
-    |x s|); its square then by 4 u |Delta_d| (|c_d| + |x_d|) s_d, and the D fused multiply-adds add at most (D + 2) u r2.
-    By Cauchy-Schwarz the sum over d is at most 4 u sqrt(r2) (|c s| + |x s|) + (D + 2) u r2, which moves k by |dk/dr2|
-    times that.  On top: GEN_EVAL_U = 24 u amp2 for the evaluation itself (sqrt.approx and ex2.approx at most 2 ulp each,
+    SIMT generator (kxt_kernel; the same form holds for the fused generators of predict.cu and cross_mean): the bound of
+    helpers.gen_bound, whose GEN_EVAL_U = 24 u amp2 covers the evaluation (sqrt.approx and ex2.approx at most 2 ulp each,
     the rounding of their arguments at most 2.3 u of k, three roundings of the polynomial, the amp2 2^ea product) and
     the fp16 (hi, lo) pair (2^-22 = 4 u).
     Tensor-core generator (kxt_tc.cu): q_d = (x_d - c_d)^2 in the difference form (3 u), its fp16 pair (4 u), w = 1/ls^2
@@ -112,10 +88,9 @@ def _kx_ref(P, C, s, tc_gen=False, u=U32):
     a2 = P["amp2"][s]
     K = a2 * _kern(P["kind"], r2)
     if tc_gen:
-        dr2 = 40.0 * r2
+        gb = u * a2 * (GEN_EVAL_U + 1.01 * _dkern(P["kind"], r2) * 40.0 * r2)
     else:
-        dr2 = 4.0 * np.sqrt(r2) * (nc[:, None] + nx[None, :]) + (P["D"] + 2.0) * r2
-    gb = u * a2 * (GEN_EVAL_U + 1.01 * _dkern(P["kind"], r2) * dr2)
+        gb = gen_bound(P["kind"], r2, nc[:, None], nx[None, :], P["D"], a2, u)
     return K, gb
 
 
@@ -126,39 +101,6 @@ def _scale_exp(x):
 
 def _ea(a2):
     return _scale_exp(np.float32(np.float32(a2) * np.float32(1.000001)))
-
-
-class Worst(object):
-    """The largest value per key, recorded once at the end of a test."""
-
-    def __init__(self, rec):
-        self.rec, self.v = rec, {}
-
-    def __call__(self, key, val):
-        self.v[key] = max(self.v.get(key, 0.0), float(val))
-
-    def flush(self):
-        for k, v in sorted(self.v.items()):
-            self.rec(k, v)
-
-
-def _same(a, b):
-    """Bit for bit, the NaNs of the untouched entries j >= M included."""
-    return a.shape == b.shape and np.array_equal(a, b, equal_nan=True)
-
-
-def _frac(err, bound, what):
-    """max err / bound, every entry within its bound (an entry whose bound is 0 must be exact)."""
-    err = np.atleast_1d(np.asarray(err, dtype=np.float64))       # argwhere of a 0-d array finds nothing
-    bound = np.broadcast_to(np.asarray(bound, dtype=np.float64), err.shape)
-    assert np.all(np.isfinite(err)), "%s: non-finite entries" % what
-    zero = bound == 0
-    assert not np.any(err[zero]), "%s: an entry with a zero bound is not exact" % what
-    f = float((err[~zero] / bound[~zero]).max()) if np.any(~zero) else 0.0
-    bad = np.argwhere(err > bound)
-    assert bad.size == 0, "%s: %d entries above the bound, first %s, worst %.3g x the bound" % (what, len(bad),
-                                                                                              bad[0].tolist(), f)
-    return f
 
 
 # ---------------------------------------------------------------------------------------------------- device plumbing
