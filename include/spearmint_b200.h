@@ -85,12 +85,12 @@ int smk_potrf_lower_batched_f64(int Npad, int S, double* A, double* winv, int* i
  *    laid out y[f*ldy + n] (F columns, each contiguous), ldy >= N.
  * alpha: [S][F][Npad] (padding zero).  sum_log_diag[s] = sum_i log L_ii;  quad[s][f] = r' K^-1 r.
  * mean[s] is subtracted from every rhs (may be NULL).  alpha / sum_log_diag / quad may be NULL.
- * N < Npad solves against the leading N x N block of the factor: rows >= N of L do not reach the result.
- * One CTA per (sample, group of right-hand sides) holds that group in shared memory; where it does not fit (Npad >
- * 14080, float32 and float64) the call runs smk_chol_solve_gm_* instead, with its contract.
+ * N < Npad solves against the leading N x N block of the factor: only rows < N of L and winv are read, so rows >= N
+ * of a joint factor may hold anything, NaN included (both entries).
+ * One CTA per (sample, group of right-hand sides) holds that group in shared memory, one launch; where it does not fit
+ * (Npad > 14080, float32 and float64) the call runs smk_chol_solve_gm_* instead, with its contract.
  * smk_chol_solve_gm_*: the same solve with the right-hand sides in global memory, at any Npad.  alpha is its working
- *   vector and must not be NULL (-11).  Only rows < N of L and winv are read, so rows >= N of a joint factor may hold
- *   anything, NaN included.  About 2 * ceil(N / NB) launches on `stream`.                                          */
+ *   vector and must not be NULL (-11).  About 2 * ceil(N / NB) launches on `stream`.                                */
 int smk_chol_solve_f32(int N, int Npad, int S, int F, const float* L, const float* winv,
                        const float* y, long long y_stride, int ldy, const float* mean,
                        float* alpha, float* sum_log_diag, float* quad, void* stream);

@@ -53,7 +53,9 @@ __global__ void __launch_bounds__(256) chol_solve_kernel(int N, int Npad, int F,
   const int warp = tid >> 5, lane = tid & 31;
   const T* Ls = L + (long)s * Npad * Npad;
   const T* Ws = winv + (long)s * (Npad / NB) * NB * NB;
-  const int nblk = Npad / NB;
+  // Only the block steps that hold rows < N run, and only rows < N of L and winv are read below the diagonal: under
+  // n_lead (N < Npad) the rows >= N belong to a larger joint factor and may hold anything, NaN included.
+  const int nblk = (N + NB - 1) / NB;
   const T mu = mean ? mean[s] : T(0);
 
   for (int n = tid; n < Npad; n += 256)
@@ -117,7 +119,8 @@ __global__ void __launch_bounds__(256) chol_solve_kernel(int N, int Npad, int F,
 
   // Rows >= N are outside the (leading) system being solved: when L is the factor of a larger joint
   // matrix (observed + pending, OPT:574 "use the sub-Cholesky") they hold joint-factor rows, not the
-  // identity, so their forward values must not leak into the quadratic form or the backward pass.
+  // identity, so their forward values (rows >= N of the last block step) must not leak into the quadratic
+  // form or the backward pass.
   for (int n = N + tid; n < Npad; n += 256)
 #pragma unroll
     for (int r = 0; r < RB; ++r) x[r * Npad + n] = T(0);
@@ -148,10 +151,10 @@ __global__ void __launch_bounds__(256) chol_solve_kernel(int N, int Npad, int F,
     T p[RB];
 #pragma unroll
     for (int r = 0; r < RB; ++r) p[r] = T(0);
-    // phase A: sum over rows k below the block of L[k, base+i] * a[k]
+    // phase A: sum over rows base+NB <= k < N of L[k, base+i] * a[k]
     const T* Lc = Ls + base + i;
     int k = base + NB + g;
-    for (; k + 3 * NG < Npad; k += 4 * NG) {
+    for (; k + 3 * NG < N; k += 4 * NG) {
       T l0 = Lc[(long)k * Npad], l1 = Lc[(long)(k + NG) * Npad], l2 = Lc[(long)(k + 2 * NG) * Npad],
         l3 = Lc[(long)(k + 3 * NG) * Npad];
 #pragma unroll
@@ -162,7 +165,7 @@ __global__ void __launch_bounds__(256) chol_solve_kernel(int N, int Npad, int F,
         p[r] = fma(l3, x[r * Npad + k + 3 * NG], p[r]);
       }
     }
-    for (; k < Npad; k += NG) {
+    for (; k < N; k += NG) {
       T l0 = Lc[(long)k * Npad];
 #pragma unroll
       for (int r = 0; r < RB; ++r) p[r] = fma(l0, x[r * Npad + k], p[r]);
@@ -179,11 +182,12 @@ __global__ void __launch_bounds__(256) chol_solve_kernel(int N, int Npad, int F,
       }
     }
     __syncthreads();
-    // phase B: a[base+i] = sum_{k>=i} W_II[k, i] * tt[k]
+    // phase B: a[base+i] = sum_{i<=k, base+k<N} W_II[k, i] * tt[k]  (0 for the rows >= N of the last block step;
+    // rows >= N of W_II are masked rather than cut from the loop: the constant trip bound keeps the float64 loop as fast)
 #pragma unroll
     for (int r = 0; r < RB; ++r) p[r] = T(0);
     for (int kk = i + g; kk < NB; kk += NG) {
-      T w = Wb[(long)kk * NB + i];
+      T w = base + kk < N ? Wb[(long)kk * NB + i] : T(0);
 #pragma unroll
       for (int r = 0; r < RB; ++r) p[r] = fma(w, tt[r * NB + kk], p[r]);
     }

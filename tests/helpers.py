@@ -1,8 +1,10 @@
 """Shared helpers of the tests: golden fixture loading, the inputs of the EI grid pass built as Factor builds them, the
-host-side measures of a factorisation's error, and the float64 kernel references with their a-priori bounds."""
+host-side measures of a factorisation's and a triangular solve's error, and the float64 kernel references with their
+a-priori bounds."""
 import os
 
 import numpy as np
+import scipy.linalg as spla
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 U32, U64 = 2.0 ** -24, 2.0 ** -53          # unit roundoff of float32 and float64
@@ -136,6 +138,101 @@ def factor_path(path, A, Np):
             check(L.smk_trtri_split_f32(Npad, Np, S, ptr(A), ptr(out["winv"]), ptr(out["hi"]), ptr(out["lo"]), ptr(wt),
                                         nb_t, st), "trtri_split")
     out["info"] = info.cpu().numpy()           # read back: nothing of this call is in flight afterwards
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------- triangular solve
+SOLVE_U = {"f32": U32, "f64": U64}
+SOLVE_NB = {"f32": 128, "f64": 64}         # diagonal blocks of the factor and of winv (Cfg<T>::NB)
+
+
+def gp_factor(eng, N, S, seed, Ntot=None, kind="Matern52", D=4, noise=1e-2):
+    """The factor of amp2 (k + 1e-6 I) + noise I over Ntot >= N points (bench.synth's hyper-samples), as Factor builds it,
+    by smk_potrf_lower_batched_*.  Returns (A (=L, lower), winv, hb, y [Ntot] standardised); every sample is checked
+    positive definite (info == 0)."""
+    import torch
+    from spearmint_b200.engine import check, fn, ptr
+    Ntot = Ntot or N
+    X, y, rs = data(Ntot, D, seed)
+    hb = eng.hypers(synth_hypers(rs, S, D, noise), kind)
+    Npad, nb = (Ntot + 127) // 128 * 128, SOLVE_NB["f32" if eng.dtype == torch.float32 else "f64"]
+    A = cov_inputs(eng, kind, X, hb, Npad)
+    winv = torch.full((S, Npad // nb, nb, nb), float("nan"), dtype=eng.dtype, device=eng.device)
+    info = torch.full((S,), -1, dtype=torch.int32, device=eng.device)
+    check(fn("smk_potrf_lower_batched", eng.dtype)(Npad, S, ptr(A), ptr(winv), ptr(info), cur_stream()), "potrf")
+    assert not np.any(info.cpu().numpy())
+    return A, winv, hb, y
+
+
+def lmul(Lh, x, trans, absval=False):
+    """float64 L x or L^T x for the lower triangular host matrix Lh [N][N] (element type), in row chunks."""
+    N = x.shape[0]
+    out = np.zeros_like(x)
+    for r0 in range(0, N, 2048):
+        Lc = Lh[r0:r0 + 2048].astype(np.float64)
+        if absval:
+            Lc = np.abs(Lc)
+        if trans:
+            out += Lc.T.dot(x[r0:r0 + 2048])
+        else:
+            out[r0:r0 + 2048] = Lc.dot(x)
+    return out
+
+
+def berr(Lh, b, a, u):
+    """max_i |b - L L^T a|_i / (u (|L||L^T||a|)_i) over the columns of b / a ([N][k], float64)."""
+    r = np.abs(b - lmul(Lh, lmul(Lh, a, True), False))
+    d = lmul(Lh, lmul(Lh, np.abs(a), True, True), False, True)
+    if np.any((d == 0) & (r != 0)) or not np.all(np.isfinite(r)):
+        return np.inf
+    m = d > 0
+    return float((r[m] / d[m]).max() / u)
+
+
+def skeel_blocks(Lh, W, N, nb):
+    """max over diagonal blocks of || |W_b| |L_bb| ||_inf on the rows < N."""
+    c = 1.0
+    for b in range((N + nb - 1) // nb):
+        n = min(nb, N - b * nb)
+        Lb = np.abs(Lh[b * nb:b * nb + n, b * nb:b * nb + n].astype(np.float64))
+        Wb = np.abs(np.tril(W[b][:n, :n]).astype(np.float64))
+        c = max(c, float(Wb.dot(Lb).sum(axis=1).max()))
+    return c
+
+
+def check_solve(prec, Lh, W, b, alpha, quad, sld, tag):
+    """One sample of smk_chol_solve(_gm)_* against scipy on the device's own L (Lh [N][N], element type; W its winv).
+    b [N][k] as the device forms it (element type); alpha [N][k] (device) or None; quad [k] or None; sld scalar or None.
+    Bounds, stated before running:
+      alpha: componentwise backward error of the two substitutions <= max(32 x scipy's, 4 (N + NB c)), c the Skeel
+             condition of the diagonal blocks (the solve applies the stored block inverses W_b);
+      quad:  relative to scipy's |L^-1 b|^2 within max(32 x scipy's own inconsistency |t|^2 - b.alpha, 4 N u);
+      sld:   within 4 N u sum |log L_ii| of the float64 sum.
+    Returns the measured fraction of each bound checked: {"alpha", "quad", "sld"}."""
+    u, N, nb = SOLVE_U[prec], b.shape[0], SOLVE_NB[prec]
+    t_sp = spla.solve_triangular(Lh, b, lower=True, check_finite=False)
+    a_sp = spla.solve_triangular(Lh, t_sp, lower=True, trans="T", check_finite=False)
+    b64 = b.astype(np.float64)
+    out = {}
+    if alpha is not None:
+        r_gpu = berr(Lh, b64, alpha.astype(np.float64), u)
+        r_sp = berr(Lh, b64, a_sp.astype(np.float64), u)
+        bound = max(32.0 * r_sp, 4.0 * (N + nb * skeel_blocks(Lh, W, N, nb)))
+        print("%s: backward error %.3g u (scipy %.3g u, bound %.3g u)" % (tag, r_gpu, r_sp, bound))
+        assert r_gpu <= bound, "%s: backward error %.3g u (scipy %.3g, bound %.3g)" % (tag, r_gpu, r_sp, bound)
+        out["alpha"] = r_gpu / bound
+    if quad is not None:
+        q_sp = (t_sp.astype(np.float64) ** 2).sum(axis=0)
+        incons = np.abs(q_sp - (b64 * a_sp.astype(np.float64)).sum(axis=0)) / q_sp
+        err = np.abs(quad - q_sp) / q_sp
+        qb = np.maximum(32.0 * incons, 4.0 * N * u)
+        assert np.all(err <= qb), (tag, err, incons)
+        out["quad"] = float((err / qb).max())
+    if sld is not None:
+        d = np.log(np.diag(Lh).astype(np.float64))
+        sb = 4.0 * N * u * np.abs(d).sum() + 1e-300
+        assert abs(sld - d.sum()) <= sb, (tag, sld, d.sum())
+        out["sld"] = abs(sld - d.sum()) / sb
     return out
 
 

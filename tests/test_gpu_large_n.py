@@ -15,7 +15,8 @@ quad must agree with scipy's |L^-1 b|^2 within max(32 x scipy's own inconsistenc
 sum_log_diag with the float64 sum within 4 N u sum |log L_ii|.  Padding rows of alpha must be zero.
 
 Bitwise invariants: the public entry above the limit equals smk_chol_solve_gm_*; a batch item equals the same sample
-solved alone; rows >= N of a joint factor (L and winv) filled with NaN change nothing under n_lead; one float32 batch
+solved alone; rows >= N of a joint factor (L and winv) filled with NaN change nothing under n_lead (at n_lead = 2040 for
+the shared-memory kernel as well; test_gpu_solve.py covers the sizes below the limit); one float32 batch
 whose last item starts more than 2^31 elements in.
 
 Callers at N = 14 209 (above both limits) against the float64 oracle: the float64 grid pass with 3 pending points
@@ -26,21 +27,15 @@ import functools
 
 import numpy as np
 import pytest
-import scipy.linalg as spla
 
-from tests.helpers import cov_inputs as _inputs, cur_stream as _stream, data as _data, synth_hypers as _hypers
+from tests.helpers import (SOLVE_NB as NBS, check_solve as _check_solve, cur_stream as _stream, data as _data,
+                           gp_factor as _gp_factor)
 
 pytestmark = pytest.mark.gpu
 
-U = {"f32": 2.0 ** -24, "f64": 2.0 ** -53}
-NBS = {"f32": 128, "f64": 64}
 NLIM = {"f32": 14080, "f64": 14080}      # the largest Npad the shared-memory kernel takes
 KIND = "Matern52"
 NX = 14209                               # Npad = 14336
-
-
-def _npad(N):
-    return (N + 127) // 128 * 128
 
 
 @pytest.fixture(scope="module")
@@ -53,21 +48,9 @@ def engs():
 # ---------------------------------------------------------------------------------------------------- device plumbing
 @functools.lru_cache(maxsize=1)
 def _factored(prec, N, S, seed, Ntot=None):
-    """The factor of amp2 (k + 1e-6 I) + noise I over Ntot >= N points (D = 4, noise 1e-2), as Factor builds it, by
-    smk_potrf_lower_batched_*.  Returns (eng, A (=L, lower), winv, hb, y [Ntot] standardised)."""
-    import torch
-    from spearmint_b200.engine import check, fn, ptr
+    """helpers.gp_factor (Matern52, D = 4, noise 1e-2) on the module's engine of prec: (eng, A, winv, hb, y)."""
     eng = _engs[prec]
-    Ntot = Ntot or N
-    X, y, rs = _data(Ntot, 4, seed)
-    hb = eng.hypers(_hypers(rs, S, 4, 1e-2), KIND)
-    Npad, nb = _npad(Ntot), NBS[prec]
-    A = _inputs(eng, KIND, X, hb, Npad)
-    winv = torch.full((S, Npad // nb, nb, nb), float("nan"), dtype=eng.dtype, device=eng.device)
-    info = torch.full((S,), -1, dtype=torch.int32, device=eng.device)
-    check(fn("smk_potrf_lower_batched", eng.dtype)(Npad, S, ptr(A), ptr(winv), ptr(info), _stream()), "potrf")
-    assert not np.any(info.cpu().numpy())
-    return eng, A, winv, hb, y
+    return (eng,) + _gp_factor(eng, N, S, seed, Ntot, KIND)
 
 
 _engs = {}
@@ -95,64 +78,6 @@ def _solve(entry, eng, N, Npad, S, F, L, winv, y, y_stride, ldy, mean, scalars=T
 def _same(a, b):
     import torch
     return all((x is None and y is None) or torch.equal(x, y) for x, y in zip(a, b))
-
-
-# ---------------------------------------------------------------------------------------------------- host references
-def _lmul(Lh, x, trans, absval=False):
-    """float64 L x or L^T x for the lower triangular host matrix Lh [N][N] (element type), in row chunks."""
-    N = x.shape[0]
-    out = np.zeros_like(x)
-    for r0 in range(0, N, 2048):
-        Lc = Lh[r0:r0 + 2048].astype(np.float64)
-        if absval:
-            Lc = np.abs(Lc)
-        if trans:
-            out += Lc.T.dot(x[r0:r0 + 2048])
-        else:
-            out[r0:r0 + 2048] = Lc.dot(x)
-    return out
-
-
-def _berr(Lh, b, a, u):
-    """max_i |b - L L^T a|_i / (u (|L||L^T||a|)_i) over the columns of b / a ([N][k], float64)."""
-    r = np.abs(b - _lmul(Lh, _lmul(Lh, a, True), False))
-    d = _lmul(Lh, _lmul(Lh, np.abs(a), True, True), False, True)
-    if np.any((d == 0) & (r != 0)) or not np.all(np.isfinite(r)):
-        return np.inf
-    m = d > 0
-    return float((r[m] / d[m]).max() / u)
-
-
-def _skeel_blocks(Lh, W, N, nb):
-    """max over diagonal blocks of || |W_b| |L_bb| ||_inf on the rows < N."""
-    c = 1.0
-    for b in range((N + nb - 1) // nb):
-        n = min(nb, N - b * nb)
-        Lb = np.abs(Lh[b * nb:b * nb + n, b * nb:b * nb + n].astype(np.float64))
-        Wb = np.abs(np.tril(W[b][:n, :n]).astype(np.float64))
-        c = max(c, float(Wb.dot(Lb).sum(axis=1).max()))
-    return c
-
-
-def _check_solve(prec, Lh, W, b, alpha, quad, sld, tag):
-    """alpha [N][k] (device), b [N][k] as the device forms it (element type); quad [k] or None; sld scalar or None."""
-    u, N = U[prec], b.shape[0]
-    t_sp = spla.solve_triangular(Lh, b, lower=True, check_finite=False)
-    a_sp = spla.solve_triangular(Lh, t_sp, lower=True, trans="T", check_finite=False)
-    b64 = b.astype(np.float64)
-    r_gpu = _berr(Lh, b64, alpha.astype(np.float64), u)
-    r_sp = _berr(Lh, b64, a_sp.astype(np.float64), u)
-    bound = max(32.0 * r_sp, 4.0 * (N + NBS[prec] * _skeel_blocks(Lh, W, N, NBS[prec])))
-    print("%s: backward error %.3g u (scipy %.3g u, bound %.3g u)" % (tag, r_gpu, r_sp, bound))
-    assert r_gpu <= bound, "%s: backward error %.3g u (scipy %.3g, bound %.3g)" % (tag, r_gpu, r_sp, bound)
-    if quad is not None:
-        q_sp = (t_sp.astype(np.float64) ** 2).sum(axis=0)
-        incons = np.abs(q_sp - (b64 * a_sp.astype(np.float64)).sum(axis=0)) / q_sp
-        err = np.abs(quad - q_sp) / q_sp
-        assert np.all(err <= np.maximum(32.0 * incons, 4.0 * N * u)), (tag, err, incons)
-    if sld is not None:
-        d = np.log(np.diag(Lh).astype(np.float64))
-        assert abs(sld - d.sum()) <= 4.0 * N * u * np.abs(d).sum() + 1e-300, (tag, sld, d.sum())
 
 
 def _cols(F):
@@ -225,17 +150,20 @@ def test_solve_gm_identity_rhs_at_size():
 
 
 @pytest.mark.parametrize("prec", ["f32", "f64"])
-@pytest.mark.parametrize("n_lead,P", [(2040, 10), (NX, 3)])
-def test_joint_factor_leading_block_and_fantasy_layout(prec, n_lead, P):
-    """A joint factor of n_lead + P points.  (1) The fantasy layout: all N + P rows, F = 3, y_stride = F (N + P),
-    ldy = N + P, mean NULL.  (2) n_lead: the leading block with the mean subtracted; then rows >= n_lead of L and of
-    winv are set to NaN and the result must not change by a bit."""
+@pytest.mark.parametrize("n_lead,P,entry", [pytest.param(2040, 10, "smk_chol_solve_gm", id="2040-10"),
+                                            pytest.param(2040, 10, "smk_chol_solve", id="2040-10-smem"),
+                                            pytest.param(NX, 3, "smk_chol_solve", id="14209-3")])
+def test_joint_factor_leading_block_and_fantasy_layout(prec, n_lead, P, entry):
+    """A joint factor of n_lead + P points, solved by `entry` (at n_lead = 2040 both the global-memory entry and the
+    public one, which runs the shared-memory kernel there; above the limit the public one runs the global-memory
+    kernel).  (1) The fantasy layout: all N + P rows, F = 3, y_stride = F (N + P), ldy = N + P, mean NULL.  (2) n_lead:
+    the leading block with the mean subtracted; then rows >= n_lead of L and of winv are set to NaN and the result must
+    not change by a bit."""
     import torch
     Nt = n_lead + P
     eng, A, winv, hb, y = _factored(prec, n_lead, 2, 11, Nt)
     A, winv = A.clone(), winv.clone()
     S, Npad, nb, F = 2, A.shape[-1], NBS[prec], 3
-    entry = "smk_chol_solve" if Npad > NLIM[prec] else "smk_chol_solve_gm"
     rs = np.random.RandomState(5)
     fant = rs.randn(S, F, Nt)
     fd = eng.to_dev(fant)
