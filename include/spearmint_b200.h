@@ -122,6 +122,18 @@ size_t smk_potrf_loglik_workspace_bytes(int Npad, int S);
 int smk_potrf_loglik_f64(int Npad, int S, double* A, void* workspace, size_t workspace_bytes, int* info, int use_graph,
                          void* stream);
 
+/* ---- (3d) the whole log-likelihood of a small GP in one launch, one CTA per item: (3) cov_build_lower, (3b)
+ * set_rhs, (3c) and (3b) finish fused, the augmented (N+1) x (N+1) lower triangle packed in shared memory.
+ * X: [N][D]; per item b: inv_ls[b][D], amp2[b], noise[b], mean[b]; y: [N].  Writes sum_log_diag[b], quad[b] as (3b)
+ * and info[b] as (2) (then sum_log_diag[b] = quad[b] = NaN).  N <= SMK_LOGLIK_SMALL_MAX_N: the largest N whose packed
+ * triangle (plus 272 doubles of scratch) fits in the 227 KB of shared memory an H100 block can opt into.  Per-item
+ * results are bitwise independent of B and of the item's position.  Never allocates, never synchronises; a bad argument
+ * #k returns -k.                                                                                                      */
+#define SMK_LOGLIK_SMALL_MAX_N 238
+int smk_loglik_small_f64(int kind, int N, int D, int B, const double* X, const double* inv_ls, const double* amp2,
+                         const double* noise, const double* mean, const double* y, double* sum_log_diag, double* quad,
+                         int* info, void* stream);
+
 /* ---- (4) fused predict: cross-covariance tiles generated on the fly -> blocked triangular
  *          solve against L -> predictive mean and variance.  beta and Kx never reach HBM as
  *          N x M matrices.            (OPT:535 cand_cross, OPT:544 beta, OPT:547-548 func_m/func_v)

@@ -53,6 +53,7 @@ SIGNATURES = {
     "smk_ei_over_hypers_host_f32": ([_i, _i, _i, _i, _i] + [_p] * 9, _i),
     "smk_potrf_loglik_workspace_bytes": ([_i, _i], _sz),
     "smk_potrf_loglik_f64": ([_i, _i, _p, _p, _sz, _p, _i, _p], _i),
+    "smk_loglik_small_f64": ([_i] * 4 + [_p] * 10, _i),
     "smk_tc_guard_workspace_bytes": ([_i, _i], _sz),
     "smk_tc_guard_f32": ([_i] * 4 + [_p] * 8 + [_sz, _p], _i),
     "smk_ei_colsum": ([_i, _i, _p, _i, _p, _p], _i),

@@ -1,6 +1,7 @@
 """Compute backend of the chooser plugins: everything numerical that ``next()`` needs, on the GPU.
 
-    loglik(kind, comp, vals)                      -> callable(mean, noise, amp2, ls) -> float   (float64, f2)
+    loglik(kind, comp, vals, chains=1)            -> callable(mean, noise, amp2, ls) -> float   (float64, f2)
+                                                     with .batch(items); chains > 1: one round of lockstep chains
     optimize_hypers(kind, comp, vals)             -> (mean, noise, amp2, ls)  ML-II, GP.optimize_hypers   (f3)
     grid_state(kind, hyper_samples, comp, pend, vals, normals, time_hs, durs_log) -> state
     ei_matrix(state, cand)                        -> (M, S) float64 numpy                        (OPT:331-341)
@@ -19,7 +20,8 @@ can be unit-tested on a CPU-only box with a stand-in backend supplied by the tes
 
 Multi-GPU: when torch.distributed is initialised (one process per GPU, NCCL), the hyper-samples of the grid pass are
 sharded round-robin over ranks and combined with ONE all-reduce of the per-candidate EI sum (parallel.py); the MCMC
-chain and the L-BFGS refinement are replicated (same seeds -> identical on every rank).
+chain and the L-BFGS refinement are replicated (same seeds -> identical on every rank).  With mcmc_chains=K > 1, chain c
+runs on rank c mod W and the finished chains are exchanged in one all-gather (chains.py).
 """
 import numpy as np
 import torch
@@ -55,8 +57,9 @@ class DeviceBackend(object):
         return self.eng64 if getattr(self, "grid_dtype", "float32") == "float64" else self.eng32
 
     # ---- f2
-    def loglik(self, kind, comp, vals):
-        return self.eng64.loglik(kind, comp, vals)
+    def loglik(self, kind, comp, vals, chains=1):
+        """chains > 1: the handle of that many lockstep chains (engine.ChainLogLik); 1: the single chain's."""
+        return self.eng64.loglik(kind, comp, vals, chains)
 
     # ---- f3: ML-II hyper-parameters (gp.GP.optimize_hypers, GP:181-292)
     def optimize_hypers(self, kind, comp, vals):

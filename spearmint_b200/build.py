@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libspearmint_b200.so")
-SOURCES = ["cov.cu", "potrf.cu", "potrf_ll.cu", "solve.cu", "predict.cu", "predict_mma.cu", "predict_tc.cu", "kxt_tc.cu", "guard.cu", "sobol.cu", "ei.cu", "grad.cu", "constraint.cu",
+SOURCES = ["cov.cu", "potrf.cu", "potrf_ll.cu", "loglik_small.cu", "solve.cu", "predict.cu", "predict_mma.cu", "predict_tc.cu", "kxt_tc.cu", "guard.cu", "sobol.cu", "ei.cu", "grad.cu", "constraint.cu",
            "forest.cu", "api.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

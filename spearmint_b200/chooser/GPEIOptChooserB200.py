@@ -14,7 +14,17 @@ evaluation is a hand-written sm_90a kernel behind the C ABI (``spearmint_b200.ba
                              (the reference re-factors K for every sample at every evaluation)
 ``use_multiprocessing`` is accepted and ignored: a forked pool cannot share a CUDA context, and with cached
 factors the 20 refinements are cheap.  Extra optional keys: ``device``, ``refine_dtype``, ``grid_dtype``,
-``state_name``.
+``state_name``, ``mcmc_chains``.
+
+``mcmc_chains=K`` (default 1) runs K independent chains of the same sampler in lockstep (chains.py): one batched
+log-likelihood call per round for all of them, and under torchrun chain c on rank c mod W.  Each chain burns in on its
+first call and then takes mcmc_iters / K steps; hyper_samples is round-major (step r of chain 0, of chain 1, ...).  The
+chains draw from RandomStates of their own, seeded by K draws of npr.randint(2**32) from the global RNG right after the
+jitter cloud of the next() that creates them; afterwards they never touch the global RNG.  The state pickle keeps the
+reference's keys (mean/noise/amp2/ls: the last chain's last sample) and adds ``chains``: per chain (mean, noise, amp2,
+ls, RandomState state).  A pickle with ``chains`` resumes without burn-in (its length must be K); one without starts
+every chain from its hyper-parameters and burns each one in.  K = 1 is the reference's single chain, unchanged (it
+reads the reference's keys of any pickle and ignores ``chains``).
 """
 import time
 
@@ -22,7 +32,7 @@ import numpy as np
 import numpy.random as npr
 import scipy.optimize as spo
 
-from spearmint_b200 import util
+from spearmint_b200 import chains, util
 from spearmint_b200.chooser._gp import GPChooser, GPPrior, read_state, write_state, write_stats
 from spearmint_b200.locker import log
 
@@ -37,9 +47,16 @@ class GPEIOptChooserB200(GPChooser):
 
     def __init__(self, expt_dir, covar="Matern52", mcmc_iters=10, pending_samples=100, noiseless=False, burnin=100,
                  grid_subset=20, use_multiprocessing=True, device=None, refine_dtype="float64", state_name=None,
-                 backend=None, grid_dtype="float32"):
+                 backend=None, grid_dtype="float32", mcmc_chains=1):
         GPChooser.__init__(self, expt_dir, covar, mcmc_iters, pending_samples, noiseless, state_name, device, backend,
                            refine_dtype, grid_dtype)
+        self.mcmc_chains = int(mcmc_chains)
+        if self.mcmc_chains < 1:
+            raise ValueError("mcmc_chains must be at least 1, got %d" % self.mcmc_chains)
+        if self.mcmc_iters > 0 and self.mcmc_iters % self.mcmc_chains:
+            raise ValueError("mcmc_iters (%d) must be a multiple of mcmc_chains (%d)" % (self.mcmc_iters,
+                                                                                       self.mcmc_chains))
+        self.chains = None          # mcmc_chains > 1: the chains.Chain list, made by the first next() or a resume
         self.burnin = int(burnin)
         self.needs_burnin = True
         self.grid_subset = int(grid_subset)
@@ -49,14 +66,22 @@ class GPEIOptChooserB200(GPChooser):
 
     # ------------------------------------------------------------------ state files (OPT:84-120, 150-205)
     def dump_hypers(self):
-        write_state(self.locker, self.state_pkl, {"dims": self.D, "ls": self.ls, "amp2": self.amp2, "noise": self.noise,
-                                                  "hyper_samples": self.hyper_samples, "mean": self.mean})
+        state = {"dims": self.D, "ls": self.ls, "amp2": self.amp2, "noise": self.noise,
+                 "hyper_samples": self.hyper_samples, "mean": self.mean}
+        if self.chains is not None:
+            state["chains"] = [c.state() for c in self.chains]
+        write_state(self.locker, self.state_pkl, state)
         write_stats(self.stats_file, self.hyper_samples)
 
     def _load_state(self, state):
         self._load_hypers(state)
         self.hyper_samples = state["hyper_samples"]
         self.needs_burnin = False
+        if self.mcmc_chains > 1 and "chains" in state:
+            if len(state["chains"]) != self.mcmc_chains:
+                raise ValueError("the state pickle holds %d chains, mcmc_chains is %d" % (len(state["chains"]),
+                                                                                        self.mcmc_chains))
+            self.chains = [chains.Chain.from_state(c, st) for c, st in enumerate(state["chains"])]
 
     def generate_stats_html(self):
         state = read_state(self.state_pkl)
@@ -117,25 +142,28 @@ class GPEIOptChooserB200(GPChooser):
             t_phase.append(time.perf_counter())
             phase_ms[name] = phase_ms.get(name, 0.0) + 1e3 * (t_phase[-1] - t_phase[-2])
 
-        self._loglik = self.backend.loglik(self.covar, comp, vals)
-        if self.needs_burnin:
-            for mcmc_iter in range(self.burnin):
-                self.sample_hypers(comp, vals)
-                log("BURN %d/%d] mean: %.2f  amp: %.2f noise: %.4f  min_ls: %.4f  max_ls: %.4f"
-                    % (mcmc_iter + 1, self.burnin, self.mean, np.sqrt(self.amp2), self.noise,
-                       np.min(self.ls), np.max(self.ls)))
-            self.needs_burnin = False
+        if self.mcmc_chains > 1:
+            self._sample_chains(comp, vals)
+        else:
+            self._loglik = self.backend.loglik(self.covar, comp, vals)
+            if self.needs_burnin:
+                for mcmc_iter in range(self.burnin):
+                    self.sample_hypers(comp, vals)
+                    log("BURN %d/%d] mean: %.2f  amp: %.2f noise: %.4f  min_ls: %.4f  max_ls: %.4f"
+                        % (mcmc_iter + 1, self.burnin, self.mean, np.sqrt(self.amp2), self.noise,
+                           np.min(self.ls), np.max(self.ls)))
+                self.needs_burnin = False
 
-        self.hyper_samples = []
-        for mcmc_iter in range(self.mcmc_iters):
-            self.sample_hypers(comp, vals)
-            log("%d/%d] mean: %.2f  amp: %.2f  noise: %.4f min_ls: %.4f  max_ls: %.4f"
-                % (mcmc_iter + 1, self.mcmc_iters, self.mean, np.sqrt(self.amp2), self.noise,
-                   np.min(self.ls), np.max(self.ls)))
-        self.dump_hypers()
-        self.stats["loglik_evals"] = getattr(self._loglik, "calls", None)
-        self.stats["loglik_batches"] = getattr(self._loglik, "launch_batches", None)
-        self._loglik = None
+            self.hyper_samples = []
+            for mcmc_iter in range(self.mcmc_iters):
+                self.sample_hypers(comp, vals)
+                log("%d/%d] mean: %.2f  amp: %.2f  noise: %.4f min_ls: %.4f  max_ls: %.4f"
+                    % (mcmc_iter + 1, self.mcmc_iters, self.mean, np.sqrt(self.amp2), self.noise,
+                       np.min(self.ls), np.max(self.ls)))
+            self.dump_hypers()
+            self.stats["loglik_evals"] = getattr(self._loglik, "calls", None)
+            self.stats["loglik_batches"] = getattr(self._loglik, "launch_batches", None)
+            self._loglik = None
         lap("mcmc")
 
         b = [(0, 1)] * cand.shape[1]       # optimization bounds
@@ -204,6 +232,21 @@ class GPEIOptChooserB200(GPChooser):
         keeps one context for the whole refinement instead."""
         f, g = self._refine_context(comp, pend, vals).value_grad(cand)
         return (f, g) if compute_grad else f
+
+    def _sample_chains(self, comp, vals):
+        """mcmc_chains > 1: every chain's burn-in (first call) and mcmc_iters / K steps, in lockstep (chains.py)."""
+        K = self.mcmc_chains
+        if self.chains is None:     # no chains in the state pickle: all start from the current hyper-parameters
+            self.chains = chains.Chain.seeded(K, (self.mean, self.noise, self.amp2, self.ls))
+        ll = self.backend.loglik(self.covar, comp, vals, chains=K)
+        self.hyper_samples, rounds = chains.sample(self.chains, self.prior, ll, vals, self.noiseless, self.burnin,
+                                                   self.mcmc_iters // K)
+        self._set_current(self.hyper_samples[-1])
+        self.needs_burnin = False
+        self.dump_hypers()
+        self.stats["loglik_evals"] = getattr(ll, "calls", None)
+        self.stats["loglik_batches"] = getattr(ll, "launch_batches", None)
+        self.stats["chain_rounds"] = rounds
 
     # ------------------------------------------------------------------ hyper-parameter sampling (OPT:621-706)
     def sample_hypers(self, comp, vals):

@@ -40,6 +40,28 @@ class GPPrior(object):
     def joint(self, ll, mean, amp2, noise, ls, targets, noiseless=False):
         """Slice move over [mean, amp2, noise] (compwise=False) -> (mean, amp2, noise).  Noiseless: the noise coordinate
         is carried along (the random direction still has 3 components) but K takes 1e-3 and the noise stays 1e-3."""
+        hypers_of = self._joint_map(ls, targets, noiseless)
+        hypers = util.slice_sample(np.array([mean, amp2, noise]), util.make_logprob(ll, hypers_of), compwise=False)
+        return hypers[0], hypers[1], (1e-3 if noiseless else hypers[2])
+
+    def length_scales(self, ll, mean, noise, amp2, ls):
+        """Component-wise slice move over the length scales -> ls."""
+        return util.slice_sample(ls, util.make_logprob(ll, self._ls_map(mean, noise, amp2)), compwise=True)
+
+    # step-wise forms (util.slice_steps): the same moves drawing from a chain's own RandomState ``rs``; they yield the
+    # (mean, noise, amp2, ls) items to evaluate and expect their log-likelihoods sent back (chains.py)
+    def joint_steps(self, rs, mean, amp2, noise, ls, targets, noiseless=False, speculate=(util.SPECULATE, 0)):
+        hypers = yield from util.with_priors(
+            util.slice_steps(np.array([mean, amp2, noise]), rs, speculate, compwise=False),
+            self._joint_map(ls, targets, noiseless))
+        return hypers[0], hypers[1], (1e-3 if noiseless else hypers[2])
+
+    def length_scales_steps(self, rs, mean, noise, amp2, ls, speculate=(util.SPECULATE, 0)):
+        return (yield from util.with_priors(util.slice_steps(ls, rs, speculate, compwise=True),
+                                            self._ls_map(mean, noise, amp2)))
+
+    def _joint_map(self, ls, targets, noiseless):
+        """hypers_of of the joint move (util.CachedLogProb)."""
         vmax, vmin = np.max(targets), np.min(targets)
         noise_scale, amp2_scale, scaled = self.noise_scale, self.amp2_scale, self.noise_times_amp2
         log_amp = (lambda a: np.log(np.sqrt(a))) if self.amp2_prior_on_std else np.log
@@ -62,20 +84,17 @@ class GPPrior(object):
                 return (mean, amp2 * noise if scaled else noise, amp2, ls), (
                     np.log(np.log(1 + (noise_scale / noise) ** 2)),              # horseshoe prior on the noise
                     -0.5 * (log_amp(amp2) / amp2_scale) ** 2)                     # log-normal prior on the amplitude
+        return hypers_of
 
-        hypers = util.slice_sample(np.array([mean, amp2, noise]), util.make_logprob(ll, hypers_of), compwise=False)
-        return hypers[0], hypers[1], (1e-3 if noiseless else hypers[2])
-
-    def length_scales(self, ll, mean, noise, amp2, ls):
-        """Component-wise slice move over the length scales -> ls."""
+    def _ls_map(self, mean, noise, amp2):
+        """hypers_of of the length-scale move."""
         max_ls = self.max_ls
 
         def hypers_of(ls):
             if np.any(ls < 0) or np.any(ls > max_ls):
                 return None
             return (mean, noise, amp2, ls), ()
-
-        return util.slice_sample(ls, util.make_logprob(ll, hypers_of), compwise=True)
+        return hypers_of
 
 
 # ---------------------------------------------------------------------------------------------- state files

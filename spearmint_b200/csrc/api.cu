@@ -113,6 +113,8 @@ size_t tc_guard_workspace_bytes(int, int);
 int tc_guard(int, int, int, int, const float*, const float*, const float*, const float*, const float*, const int*, float*, void*,
              size_t, cudaStream_t);
 int potrf_ll_f64(int, int, double*, double*, int*, int, cudaStream_t);
+int loglik_small_f64(int, int, int, int, const double*, const double*, const double*, const double*, const double*,
+                     const double*, double*, double*, int*, cudaStream_t);
 size_t forest_workspace_bytes(int, int, int);
 int forest_fit(int, int, int, const float*, const double*, const double*, const uint32_t*, int, int, int, int, int*,
                double*, int*, int*, int*, double*, int*, void*, size_t, cudaStream_t);
@@ -181,6 +183,11 @@ int smk_potrf_loglik_f64(int Npad, int S, double* A, void* workspace, size_t wor
                          void* stream) {
   if (!workspace || workspace_bytes < potrf_ll_workspace_bytes(Npad, S)) return -4;
   return potrf_ll_f64(Npad, S, A, reinterpret_cast<double*>(workspace), info, use_graph, ST(stream));
+}
+int smk_loglik_small_f64(int kind, int N, int D, int B, const double* X, const double* inv_ls, const double* amp2,
+                         const double* noise, const double* mean, const double* y, double* sum_log_diag, double* quad,
+                         int* info, void* stream) {
+  return loglik_small_f64(kind, N, D, B, X, inv_ls, amp2, noise, mean, y, sum_log_diag, quad, info, ST(stream));
 }
 
 int smk_chol_solve_f32(int N, int Npad, int S, int F, const float* L, const float* winv, const float* y,

@@ -991,8 +991,8 @@ class GPEIEngine(object):
         return ei[:, :M].t().contiguous().cpu().numpy()
 
     # ------------------------------------------------------------------ f2: GP log marginal likelihood
-    def loglik(self, kind, comp, vals):
-        return LogLik(self, kind, comp, vals)
+    def loglik(self, kind, comp, vals, chains=1):
+        return LogLik(self, kind, comp, vals) if chains == 1 else ChainLogLik(self, kind, comp, vals, chains)
 
     # ------------------------------------------------------------------ classification GP of the constrained chooser
     def latent_loglik(self, kind, comp, ls, noise=CONSTRAINT_NOISE):
@@ -1090,6 +1090,57 @@ class LogLik(object):
         if np.isnan(v):
             raise np.linalg.LinAlgError("leading minor of the array is not positive definite")
         return v
+
+
+LOGLIK_SMALL_MAX_N = 238      # SMK_LOGLIK_SMALL_MAX_N of include/spearmint_b200.h
+
+
+class ChainLogLik(LogLik):
+    """The log-likelihood handle of ``chains`` lockstep chains (chains.py): one ``batch`` call per round carries the
+    outstanding items of every chain, at most chains * (3 + max speculation depth) of them.
+      N <= LOGLIK_SMALL_MAX_N : smk_loglik_small_f64, the whole evaluation in one launch (one CTA per item);
+      larger N                : LogLik's batched path with max_batch sized for a full round, so a round is one launch
+                                sequence; the potrf_loglik graph is captured once per batch size B met (no padding).
+    Per-item values are bitwise independent of the batch size and position on both paths, so a chain's draws do not
+    depend on how many chains share its rounds."""
+
+    def __init__(self, eng, kind, comp, vals, chains):
+        N = comp.shape[0]
+        self.speculate = (3, 0) if N <= 1536 else (0, 2)          # LogLik's schedule (set again by LogLik.__init__)
+        max_batch = chains * (3 + max(self.speculate))
+        self.small = N <= LOGLIK_SMALL_MAX_N
+        self.device = eng.device
+        if not self.small:
+            LogLik.__init__(self, eng, kind, comp, vals, max_batch)
+            return
+        self.eng, self.kind = eng, kind
+        self.X, self.y = eng.to_dev(comp), eng.to_dev(vals)
+        self.N, self.D = self.X.shape
+        self.max_batch = max_batch
+        self.out = torch.empty((2, max_batch), dtype=torch.float64, device=eng.device)
+        self.info = torch.zeros((max_batch,), dtype=torch.int32, device=eng.device)
+        self.calls = 0
+        self.launch_batches = 0
+
+    def batch(self, items):
+        """items: list of (mean, noise, amp2, ls).  Returns a float64 array; NaN marks a non-PD matrix."""
+        if not self.small:
+            return LogLik.batch(self, items)
+        out = np.empty(len(items))
+        for b0 in range(0, len(items), self.max_batch):
+            its = items[b0:b0 + self.max_batch]
+            B = len(its)
+            hb, y = self._chunk(its)
+            check(_lib.lib().smk_loglik_small_f64(KINDS[self.kind], self.N, self.D, B, ptr(self.X), ptr(hb.inv_ls),
+                                                  ptr(hb.amp2), ptr(hb.noise), ptr(hb.mean), ptr(y), ptr(self.out[0]),
+                                                  ptr(self.out[1]), ptr(self.info), self.eng.stream()), "loglik_small")
+            r = torch.cat([self.out[0, :B], self.out[1, :B], self.info[:B].double()]).cpu().numpy()
+            lp = -r[:B] - 0.5 * r[B:2 * B]
+            lp[r[2 * B:] != 0] = np.nan
+            out[b0:b0 + B] = lp
+            self.calls += B
+            self.launch_batches += 1
+        return out
 
 
 class RefineContext(object):

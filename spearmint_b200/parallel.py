@@ -46,6 +46,26 @@ def agree_on_error(exc, device="cpu", group=None):
         raise np.linalg.LinAlgError("a hyper-sample owned by another rank is not positive definite")
 
 
+def allgather_object(obj, device="cpu", group=None):
+    """[object of rank 0, object of rank 1, ...] on every rank: ``obj`` pickled into a byte tensor on ``device`` (the
+    rank's own GPU with NCCL, "cpu" with gloo), one all-gather of the lengths and one of the padded bytes."""
+    if not (dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1):
+        return [obj]
+    import pickle
+    import torch
+    W = dist.get_world_size(group)
+    data = torch.frombuffer(bytearray(pickle.dumps(obj, protocol=2)), dtype=torch.uint8).to(device)
+    n = torch.tensor([data.numel()], dtype=torch.int64, device=device)
+    ns = [torch.zeros_like(n) for _ in range(W)]
+    dist.all_gather(ns, n, group=group)
+    size = max(int(x[0]) for x in ns)
+    buf = torch.zeros((size,), dtype=torch.uint8, device=device)
+    buf[:data.numel()] = data
+    bufs = [torch.zeros_like(buf) for _ in range(W)]
+    dist.all_gather(bufs, buf, group=group)
+    return [pickle.loads(b[:int(k[0])].cpu().numpy().tobytes()) for b, k in zip(bufs, ns)]
+
+
 def sharded_mean_ei(local_ei_sum_fn, S, group=None):
     """mean_s EI[s, :] from per-rank partial sums.
 

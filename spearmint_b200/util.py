@@ -22,12 +22,13 @@ def unpack_args(arg_string):
 SPECULATE = 3    # shrink proposals evaluated ahead of time when the log-probability supports batching
 
 
-def _peek_shrink(lower, upper, n):
-    """The next n shrink proposals of the interval (lower, upper) assuming each one is rejected, obtained by PEEKING the
-    global RNG (state saved and restored): the draws consumed later are exactly these."""
-    state = npr.get_state()
-    peek = npr.rand(n)
-    npr.set_state(state)
+def _peek_shrink(lower, upper, n, rng=npr):
+    """The next n shrink proposals of the interval (lower, upper) assuming each one is rejected, obtained by PEEKING
+    ``rng`` (the global RNG, or a chain's RandomState; state saved and restored): the draws consumed later are exactly
+    these."""
+    state = rng.get_state()
+    peek = rng.rand(n)
+    rng.set_state(state)
     zs, lo, hi = [], lower, upper
     for r in peek:
         z = (hi - lo) * r + lo
@@ -111,6 +112,111 @@ def slice_sample(init_x, logprob, sigma=1.0, step_out=True, max_steps_out=1000, 
     direction = npr.randn(dims)
     direction = direction / np.sqrt(np.sum(direction ** 2))
     return _slice_along(direction, init_x, logprob, sigma, step_out, max_steps_out)
+
+
+# ---------------------------------------------------------------------------------------------- step-wise slice sampler
+# The same sampler as a generator, so that several chains can share one batched log-likelihood call per round
+# (chains.py).  It draws from an explicit RandomState, yields the list of points whose log-probabilities it needs, and
+# expects the list of their values sent back (NaN: the covariance is not positive definite).  Its draws, the points it
+# visits and its result are slice_sample's with a CachedLogProb of the same ``speculate`` (tests/test_mcmc_chains_host.py).
+def _not_pd():
+    return np.linalg.LinAlgError("leading minor of the array is not positive definite")
+
+
+def _lp_step(x, cache):
+    """Log-probability at ``x``: from the move's prefetched values, else one point of its own (CachedLogProb.__call__)."""
+    v = cache.get(CachedLogProb._key(x))
+    if v is None:
+        v = (yield [x])[0]
+    if np.isnan(v):
+        raise _not_pd()
+    return v
+
+
+def _prefetch_step(points):
+    """CachedLogProb.prefetch: a fresh cache holding the values of ``points``."""
+    vals = yield points
+    return {CachedLogProb._key(x): v for x, v in zip(points, vals)}
+
+
+def _slice_along_steps(direction, x0, rs, sigma, step_out, max_steps_out, speculate):
+    """_slice_along with ``rs`` for the global RNG and a prefetching log-probability of depth ``speculate``."""
+    s1, s2 = speculate
+    upper = sigma * rs.rand()
+    lower = upper - sigma
+    u_height = rs.rand()
+    zs = [0.0, lower, upper] + _peek_shrink(lower, upper, s1, rs)
+    cache = yield from _prefetch_step([direction * z + x0 for z in zs])
+    height = np.log(u_height) + (yield from _lp_step(direction * 0.0 + x0, cache))
+    n_lo = n_hi = 0
+    if step_out:
+        while (yield from _lp_step(direction * lower + x0, cache)) > height and n_lo < max_steps_out:
+            n_lo += 1
+            lower -= sigma
+        while (yield from _lp_step(direction * upper + x0, cache)) > height and n_hi < max_steps_out:
+            n_hi += 1
+            upper += sigma
+    covered = s1 if (n_lo == 0 and n_hi == 0) else 0
+    it = 0
+    while True:
+        if s2 > 0 and it >= covered:
+            cache = yield from _prefetch_step([direction * z + x0 for z in _peek_shrink(lower, upper, s2, rs)])
+            covered = it + s2
+        z = (upper - lower) * rs.rand() + lower
+        val = yield from _lp_step(direction * z + x0, cache)
+        it += 1
+        if val > height:
+            return z * direction + x0
+        if z < 0:
+            lower = z
+        elif z > 0:
+            upper = z
+        else:
+            raise Exception("Slice sampler shrank to zero!")
+
+
+def slice_steps(init_x, rs, speculate=(SPECULATE, 0), sigma=1.0, step_out=True, max_steps_out=1000, compwise=False):
+    """Generator form of slice_sample drawing from the RandomState ``rs``; its return value is the new point."""
+    init_x = np.asarray(init_x, dtype=float)
+    if not init_x.shape:
+        init_x = np.array([init_x])
+    dims = init_x.shape[0]
+    if compwise:
+        order = list(range(dims))
+        rs.shuffle(order)
+        x = init_x.copy()
+        for d in order:
+            e = np.zeros(dims)
+            e[d] = 1.0
+            x = yield from _slice_along_steps(e, x, rs, sigma, step_out, max_steps_out, speculate)
+        return x
+    direction = rs.randn(dims)
+    direction = direction / np.sqrt(np.sum(direction ** 2))
+    return (yield from _slice_along_steps(direction, init_x, rs, sigma, step_out, max_steps_out, speculate))
+
+
+def with_priors(steps, hypers_of):
+    """Runs a slice_steps generator on a log-probability made of ``hypers_of`` (CachedLogProb's map) and a GP
+    log-likelihood: yields the (mean, noise, amp2, ls) items whose log-likelihoods it needs (never an empty list),
+    expects their values sent back (NaN: not positive definite) and returns the sampler's result."""
+    try:
+        points = next(steps)
+        while True:
+            maps = [hypers_of(np.asarray(x, dtype=float)) for x in points]
+            todo = [h[0] for h in maps if h is not None]
+            lls = iter((yield todo) if todo else ())
+            lps = []
+            for h in maps:
+                if h is None:
+                    lps.append(-np.inf)
+                    continue
+                v = next(lls)
+                for t in h[1]:                   # prior terms in the reference's order of addition
+                    v = v + t
+                lps.append(v)
+            points = steps.send(lps)
+    except StopIteration as stop:
+        return stop.value
 
 
 class CachedLogProb(object):
