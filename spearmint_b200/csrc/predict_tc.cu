@@ -12,7 +12,8 @@
 //                (kxt_kernel below: SIMT, the default; kxt_tc.cu: opt-in tensor-core generator.)
 //   4. mma     : per (sample, 128-candidate tile, row-group pair):  D[c][i] = sum_n Kxt[c][n] * Linv[i][n]
 //                as 3 x FP16 (lo*hi + hi*lo + hi*hi) with wgmma m64n256k16, fp32 accumulation, operands staged by
-//                TMA (64-byte swizzle, 4 stages) by a producer warpgroup, two consumer warpgroups with the 128 x 256
+//                TMA (64-byte swizzle, 4 stages) by a producer warpgroup, in 2-CTA clusters that share every Linv tile
+//                by TMA multicast (adjacent candidate tiles), two consumer warpgroups with the 128 x 256
 //                accumulator in registers; epilogue = un-scale by 2^-(ea+eb), sum of squares per candidate row (over
 //                the 4 lanes that share a row), partial sums per row-group pair.
 //   5. finish  : var = amp2 (1 + 1e-6) - sum_p partial[p]
@@ -415,18 +416,29 @@ struct Args {
   float *xhi, *xlo, *xthi, *xtlo;   // mode 3 outputs, each [S][Np][Np]
 };
 
-// One unit of MMA work: A rows / B rows / k range (in elements) of a single accumulator pass.
-struct Item { int valid, rowA, rowB, k0, nk, s, tile, g, pr; };
+// One unit of MMA work: A rows / B rows / k range (in elements) of a single accumulator pass.  own == 0: the CTA runs
+// the item's loads and MMAs to keep its cluster in step, but writes nothing.
+struct Item { int valid, own, rowA, rowB, k0, nk, s, tile, g, pr; };
 
-__device__ __forceinline__ Item get_item(const Args& p, long w, int h) {
+// Work items of modes 0, 1 are (sample, group of CLUSTER candidate tiles, row-group pair); CTA `rank` of the cluster
+// takes tile CLUSTER * group + rank, so the CTAs of a cluster walk identical B rows and k ranges.  When the tile count is
+// not a multiple of CLUSTER, the CTAs past the last tile re-run tile ntiles - 1 without writing it.
+template <int CLUSTER>
+__device__ __forceinline__ long num_items(const Args& p) {
+  return p.mode <= 1 ? (long)p.S * ((p.ntiles + CLUSTER - 1) / CLUSTER) * p.npairs : (long)p.S * p.ntiles;
+}
+template <int CLUSTER>
+__device__ __forceinline__ Item get_item(const Args& p, long w, int h, int rank) {
   Item it;
-  it.valid = 0; it.rowA = it.rowB = it.k0 = it.nk = it.s = it.tile = it.g = it.pr = 0;
+  it.valid = 0; it.own = 1; it.rowA = it.rowB = it.k0 = it.nk = it.s = it.tile = it.g = it.pr = 0;
   const int bk = p.f16 ? BK16 : BK;
   if (p.mode <= 1) {
+    const int ntg = (p.ntiles + CLUSTER - 1) / CLUSTER;
     it.pr = (int)(w % p.npairs);
     const long st = w / p.npairs;
-    it.tile = (int)(st % p.ntiles);
-    it.s = (int)(st / p.ntiles);
+    it.tile = (int)(st % ntg) * CLUSTER + rank;
+    it.s = (int)(st / ntg);
+    if (it.tile >= p.ntiles) { it.tile = p.ntiles - 1; it.own = 0; }
     it.g = (h == 0) ? it.pr : p.ngroups - 1 - it.pr;
     if (h == 1 && (p.mode == 1 || it.g == it.pr)) return it;   // rect: one group per item; middle group of an odd count
     it.nk = (p.mode == 1) ? p.Np / bk : (it.g + 1) * (BN / bk);
@@ -454,24 +466,34 @@ __device__ __forceinline__ Item get_item(const Args& p, long w, int h) {
   return it;
 }
 
+// CLUSTER = 2 (modes 0, 1): two CTAs with adjacent candidate tiles share every B tile.  Each loads its own A tile and
+// rows [128 rank, 128 rank + 128) of the B box (mBhi / mBlo boxes of BN / 2 rows), multicast into the same stage of both
+// CTAs, so full[stage] of each CTA counts the whole 48 KB.  A producer may refill a stage only when the consumers of BOTH
+// CTAs have released it (its multicast writes into the peer), so every consumer warp arrives on empty[stage] of both.
+// CLUSTER = 1: modes 2 and 3, one CTA per item as before.
+template <int CLUSTER>
 __global__ void __launch_bounds__(THREADS, 1)
 predict_tc_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constant__ CUtensorMap mAlo,
                   const __grid_constant__ CUtensorMap mBhi, const __grid_constant__ CUtensorMap mBlo, Args p) {
+  static_assert(CLUSTER == 1 || CLUSTER == 2, "one CTA, or a pair sharing the B operand");
   extern __shared__ unsigned char smem_raw[];
   // 1 KB alignment of the operand tiles (swizzle atoms), by offset so the pointer keeps its shared address space
   unsigned char* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(base + STAGES * STAGE_BYTES);
   uint64_t* full = bars;                 // [STAGES]  TMA bytes landed: operands ready for the MMA
-  uint64_t* empty = bars + STAGES;       // [STAGES]  stage consumed by every consumer warp
+  uint64_t* empty = bars + STAGES;       // [STAGES]  stage consumed by every consumer warp of the cluster
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int rank = CLUSTER > 1 ? (int)cluster_ctarank() : 0;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CONSUMERS * 4); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], CLUSTER * CONSUMERS * 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
+  if (CLUSTER > 1) cluster_sync();       // the peer's barriers are initialised before any multicast or remote arrive
+  else __syncthreads();
 
-  const long nitems = (long)p.S * p.ntiles * (p.mode <= 1 ? p.npairs : 1);
+  const long nitems = num_items<CLUSTER>(p);
+  const long w0 = blockIdx.x / CLUSTER, dw = gridDim.x / CLUSTER;
   const int bk = p.f16 ? BK16 : BK;
   // mode 0 item order (s, tile, pair): consecutive items share (s, tile) so the pair-blocks of one candidate tile run
   // concurrently on neighbouring SMs and hit L2 for the Kxt slab.
@@ -485,9 +507,9 @@ predict_tc_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
       const uint64_t hintB = 0x14F0000000000000ull;   // EVICT_LAST : the B operand is re-read by many items
       int stage = 0;
       uint32_t phase = 0;
-      for (long w = blockIdx.x; w < nitems; w += gridDim.x) {
+      for (long w = w0; w < nitems; w += dw) {
         for (int h = 0; h < 2; ++h) {
-          const Item it = get_item(p, w, h);
+          const Item it = get_item<CLUSTER>(p, w, h, rank);
           if (!it.valid) break;
           for (int kc = 0; kc < it.nk; ++kc) {
             mbar_wait_relaxed(&empty[stage], phase ^ 1, 64);
@@ -496,13 +518,22 @@ predict_tc_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
             mbar_expect_tx(&full[stage], STAGE_BYTES);
             tma_load_2d(&mAhi, &full[stage], sb, kk, it.rowA, hintA);
             tma_load_2d(&mAlo, &full[stage], sb + A_BYTES, kk, it.rowA, hintA);
-            tma_load_2d(&mBhi, &full[stage], sb + 2 * A_BYTES, kk, it.rowB, hintB);
-            tma_load_2d(&mBlo, &full[stage], sb + 2 * A_BYTES + B_BYTES, kk, it.rowB, hintB);
+            if (CLUSTER == 1) {
+              tma_load_2d(&mBhi, &full[stage], sb + 2 * A_BYTES, kk, it.rowB, hintB);
+              tma_load_2d(&mBlo, &full[stage], sb + 2 * A_BYTES + B_BYTES, kk, it.rowB, hintB);
+            } else {
+              const int hb = rank * (BN / CLUSTER);       // this CTA's rows of the B box
+              const uint16_t all = (1u << CLUSTER) - 1;
+              tma_load_2d_multicast(&mBhi, &full[stage], sb + 2 * A_BYTES + hb * ROW_BYTES, kk, it.rowB + hb, all, hintB);
+              tma_load_2d_multicast(&mBlo, &full[stage], sb + 2 * A_BYTES + B_BYTES + hb * ROW_BYTES, kk, it.rowB + hb,
+                                    all, hintB);
+            }
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
         }
       }
     }
+    if (CLUSTER > 1) cluster_sync();     // matches the consumers' exit barrier below
     return;
   }
 
@@ -513,14 +544,20 @@ predict_tc_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const int cq = 2 * (lane & 3);
   const uint32_t a_off = (uint32_t)wg * 64 * ROW_BYTES;
+  auto release = [&](int st) {            // one arrival per consumer warp on empty[st] of every CTA of the cluster
+    if (CLUSTER == 1) mbar_arrive(&empty[st]);
+    else
+#pragma unroll
+      for (int r = 0; r < CLUSTER; ++r) mbar_arrive_cluster(&empty[st], r);
+  };
   float d[BN / 2];
   int stage = 0;
   uint32_t phase = 0;
-  for (long w = blockIdx.x; w < nitems; w += gridDim.x) {
+  for (long w = w0; w < nitems; w += dw) {
     float acc[2] = {0.f, 0.f}, accm[2] = {0.f, 0.f};
-    const Item it0 = get_item(p, w, 0);
+    const Item it0 = get_item<CLUSTER>(p, w, 0, rank);
     for (int h = 0; h < 2; ++h) {
-      const Item it = get_item(p, w, h);
+      const Item it = get_item<CLUSTER>(p, w, h, rank);
       if (!it.valid) break;
       int prev = -1;
       for (int kc = 0; kc < it.nk; ++kc) {
@@ -548,13 +585,14 @@ predict_tc_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
         }
         wgmma_commit();
         wgmma_wait<1>();                                   // the previous stage's MMAs are done: hand it back to TMA
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+        if (prev >= 0 && lane == 0) release(prev);
         prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
       wgmma_hold(d);
-      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+      if (prev >= 0 && lane == 0) release(prev);
+      if (!it.own) continue;
       // undo the exact power-of-two operand scaling of the fp16 path
       const float scl = p.f16 ? ldexpf(1.f, -(kx_exp(p.amp2[it.s]) + p.bexp[it.s])) : 1.f;
       if (p.mode == 0) {
@@ -632,7 +670,7 @@ predict_tc_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
         }
       }
     }
-    if (p.mode == 0) {             // row sums over the 4 lanes that share a row, fixed order
+    if (p.mode == 0 && it0.own) {   // row sums over the 4 lanes that share a row, fixed order
 #pragma unroll
       for (int rh = 0; rh < 2; ++rh) {
         float a = acc[rh], m = accm[rh];
@@ -648,6 +686,7 @@ predict_tc_kernel(const __grid_constant__ CUtensorMap mAhi, const __grid_constan
       }
     }
   }
+  if (CLUSTER > 1) cluster_sync();       // no remote arrive or multicast may target a CTA that has exited
 }
 
 // var = amp2 (1 + 1e-6) - sum_p partial[p]; with the tensor-core generator also mu = amp2 * sum_j mu_partial[j] + mean
@@ -683,6 +722,7 @@ __global__ void kxt_mu_finish_kernel(int M, int Mc, int S, int nmp, const float*
   for (int j = 0; j < nmp; ++j) m += mu_partial[((long)j * S + s) * Mc + c];
   mu[(long)s * ldm + c] = fmaf(amp2[s], m, mean[s]);
 }
+int num_sms();
 namespace tc {
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -725,9 +765,42 @@ static int make_map_h(CUtensorMap* m, const __half* ptr, uint64_t rows, uint64_t
                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : 2;
 }
-}  // namespace tc
 
-int num_sms();
+// Modes 0 and 1 (the predict GEMMs): persistent grid of 2-CTA clusters.  The grid is the number of clusters that can be
+// co-resident, not num_sms() / 2: a GPC whose usable SM count is odd leaves one SM without a partner, and clusters
+// beyond those that fit would run as a second wave.  The B maps must have boxes of BN / kPredictCluster rows.
+constexpr int kPredictCluster = 2;
+static int launch_predict(const CUtensorMap& mAhi, const CUtensorMap& mAlo, const CUtensorMap& mBhi,
+                          const CUtensorMap& mBlo, const Args& a, cudaStream_t st) {
+  constexpr int C = kPredictCluster;
+  auto kern = predict_tc_kernel<C>;
+  static int max_clusters = 0;
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = C;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.blockDim = dim3(THREADS);
+  cfg.dynamicSmemBytes = SMEM_BYTES;
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  if (!max_clusters) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    cfg.gridDim = dim3(C * num_sms());
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveClusters(&max_clusters, kern, &cfg);
+    if (e != cudaSuccess || max_clusters <= 0) {
+      max_clusters = 0;
+      return check_launch("predict_tc cluster occupancy");
+    }
+  }
+  const long nitems = (long)a.S * ((a.ntiles + C - 1) / C) * a.npairs;
+  cfg.gridDim = dim3((unsigned)(std::min<long>(nitems, max_clusters) * C));
+  cudaLaunchKernelEx(&cfg, kern, mAhi, mAlo, mBhi, mBlo, a);
+  return check_launch("predict_tc_kernel");
+}
+}  // namespace tc
 // tensor-core cross-covariance generator (kxt_tc.cu)
 bool kxt_tc_supported(int D, int S);
 bool kxt_tc_preferred(int D, int S);
@@ -784,7 +857,7 @@ int tc_chol_update(int Npad, int S, int jb, int ncols, float* A, const float* lh
     return 1999;
   static bool attr = false;
   if (!attr) {
-    cudaFuncSetAttribute(tc::predict_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES);
+    cudaFuncSetAttribute(tc::predict_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES);
     attr = true;
   }
   tc::Args a;
@@ -794,7 +867,7 @@ int tc_chol_update(int Npad, int S, int jb, int ncols, float* A, const float* lh
   long nitems = (long)S * a.ntiles;
   int grid = (int)std::min<long>(nitems, num_sms());
   timing_begin("tc_chol_update", st);
-  tc::predict_tc_kernel<<<grid, tc::THREADS, tc::SMEM_BYTES, st>>>(mAhi, mAlo, mBhi, mBlo, a);
+  tc::predict_tc_kernel<1><<<grid, tc::THREADS, tc::SMEM_BYTES, st>>>(mAhi, mAlo, mBhi, mBlo, a);
   timing_end(st);
   count_launch();
   return check_launch("tc_chol_update");
@@ -882,7 +955,7 @@ static int trtri_tc_run(int Npad, int Np, int S, const float* L, float* winv, fl
     return 1999;
   static bool attr = false;
   if (!attr) {
-    cudaFuncSetAttribute(tc::predict_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES);
+    cudaFuncSetAttribute(tc::predict_tc_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES);
     attr = true;
   }
   const int nblk = Npad / 128;
@@ -903,7 +976,7 @@ static int trtri_tc_run(int Npad, int Np, int S, const float* L, float* winv, fl
     a.xhi = linv_hi; a.xlo = linv_lo; a.xthi = xthi; a.xtlo = xtlo;
     long nitems = (long)S * a.ntiles;
     int grid = (int)std::min<long>(nitems, num_sms());
-    tc::predict_tc_kernel<<<grid, tc::THREADS, tc::SMEM_BYTES, st>>>(mAhi, mAlo, mBhi, mBlo, a);
+    tc::predict_tc_kernel<1><<<grid, tc::THREADS, tc::SMEM_BYTES, st>>>(mAhi, mAlo, mBhi, mBlo, a);
     count_launch(2);
   }
   timing_end(st);
@@ -1171,7 +1244,8 @@ int predict_tc(int kind, int N, int Np, int M, int D, int S, const float* X, con
     alpha_pack_f16_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(N, Np, F, Fp, Npad_alpha, total, alpha_f, fexp,
                                                                            ahi, alo);
     count_launch(2);
-    if (tc::make_map_h(&mFhi, ahi, (uint64_t)S * Fp, Np, tc::BN) || tc::make_map_h(&mFlo, alo, (uint64_t)S * Fp, Np, tc::BN))
+    if (tc::make_map_h(&mFhi, ahi, (uint64_t)S * Fp, Np, tc::BN / tc::kPredictCluster) ||
+        tc::make_map_h(&mFlo, alo, (uint64_t)S * Fp, Np, tc::BN / tc::kPredictCluster))
       return 1999;
   }
 
@@ -1182,13 +1256,9 @@ int predict_tc(int kind, int N, int Np, int M, int D, int S, const float* X, con
         tc::make_map_h(&mAlo[b], kh + kelems, (uint64_t)S * Mc, Np, tc::BM))
       return 1999;                                                              // cuTensorMapEncodeTiled failed
   }
-  if (tc::make_map_h(&mBhi, linv_hi, (uint64_t)S * Np, Np, tc::BN) || tc::make_map_h(&mBlo, linv_lo, (uint64_t)S * Np, Np, tc::BN))
+  if (tc::make_map_h(&mBhi, linv_hi, (uint64_t)S * Np, Np, tc::BN / tc::kPredictCluster) ||
+      tc::make_map_h(&mBlo, linv_lo, (uint64_t)S * Np, Np, tc::BN / tc::kPredictCluster))
     return 1999;
-  static bool attr = false;
-  if (!attr) {
-    cudaFuncSetAttribute(tc::predict_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES);
-    attr = true;
-  }
   // The cross-covariance of chunk i+1 is generated on an auxiliary stream while the MMA kernel consumes chunk i
   // (two Kxt buffers; event fork/join keeps everything ordered with respect to the caller's stream).
   static cudaStream_t aux = nullptr;
@@ -1235,10 +1305,9 @@ int predict_tc(int kind, int N, int Np, int M, int D, int S, const float* X, con
     a.M = M; a.c_begin = c_begin; a.ldm = ldm; a.mean = mean;
     a.mode = 0; a.f16 = 1; a.amp2 = amp2; a.bexp = linv_exp;
     { const char* e = getenv("SMK_TC_A_EVICT_FIRST"); a.a_evict_first = (e && e[0] == '1') ? 1 : 0; }
-    long nitems = (long)S * a.ntiles * npairs;
-    int grid = (int)std::min<long>(nitems, num_sms());
     timing_begin("predict_tc_kernel", st);
-    tc::predict_tc_kernel<<<grid, tc::THREADS, tc::SMEM_BYTES, st>>>(mAhi[b], mAlo[b], mBhi, mBlo, a);
+    int rc = tc::launch_predict(mAhi[b], mAlo[b], mBhi, mBlo, a, st);
+    if (rc) return rc;
     timing_end(st);
     tc::finish_var_kernel<<<dim3((mc_used + 255) / 256, S), 256, 0, st>>>(M, c_begin, mc_used, S, npairs, Mc, partial,
                                                                         amp2, var, ldm, nmp, mu_partial, mean, mu,
@@ -1247,10 +1316,9 @@ int predict_tc(int kind, int N, int Np, int M, int D, int S, const float* X, con
     if (fant) {      // fantasy means: same Kxt chunk against alpha^T, rectangular k range (OPT:609)
       tc::Args r = a;
       r.mode = 1; r.F = F; r.mu_f = mu_f; r.bexp = fexp; r.z = nullptr; r.ngroups = Fp / tc::BN; r.npairs = r.ngroups;
-      long nit = (long)S * r.ntiles * r.npairs;
-      int gr = (int)std::min<long>(nit, num_sms());
       timing_begin("predict_tc_kernel_rect", st);
-      tc::predict_tc_kernel<<<gr, tc::THREADS, tc::SMEM_BYTES, st>>>(mAhi[b], mAlo[b], mFhi, mFlo, r);
+      rc = tc::launch_predict(mAhi[b], mAlo[b], mFhi, mFlo, r, st);
+      if (rc) return rc;
       timing_end(st);
       count_launch();
     }

@@ -135,6 +135,36 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
       "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
       : "memory");
 }
+// tma_load_2d, written to the same shared-memory offset of every CTA of the cluster named in `mask`; the bytes are
+// counted on the mbarrier at `bar`'s offset in each of those CTAs.
+__device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1,
+                                                      uint16_t mask, uint64_t hint) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5, %6;" ::"r"(smem_u32(dst)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask), "l"(hint)
+      : "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// Arrive on the mbarrier at `bar`'s shared-memory offset in CTA `rank` of the cluster (this CTA included).  The
+// predict GEMM's consumers use it to hand a stage back after wgmma.wait_group has retired the MMAs that read it; the
+// default (CTA-scope) semantics suffice for that.  The .release.cluster form orders all of the thread's earlier memory
+// operations at cluster scope on every arrival, and made the clustered GEMM 45 % slower than the single-CTA one on H100.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
+      "r"(rank)
+      : "memory");
+}
 // ------------------------------------------------------------------------------------------------------------ wgmma
 // Shared-memory matrix descriptor of a K-major operand tile in the 64-byte swizzle (rows of 64 bytes, 8-row atoms of
 // 512 bytes: stride byte offset 512; the leading byte offset is unused for swizzled K-major tiles).  The tile base must
